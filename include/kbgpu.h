@@ -42,7 +42,9 @@ typedef enum kb_status {
   KB_E_CUDA = -3,
   KB_E_NCCL = -4,
   KB_E_STATE = -5,              /* call order violated (e.g. kb_allocate before kb_session_load) */
-  KB_E_UNSUPPORTED_FEATURE = -6 /* snapshot uses a feature outside this build (inter-pod affinity, preferred affinity) */
+  KB_E_UNSUPPORTED_FEATURE = -6 /* snapshot uses a feature outside this build; kb_last_error names it (e.g. inter-pod or preferred node
+                                   affinity on a sharded node axis, reclaim / preempt with inter-pod affinity beyond host-level
+                                   anti-affinity, an evicted affinity group member, an action after preempt) */
 } kb_status;
 
 /* node_flags bits — evaluated once by the flattener from v1.Node
@@ -209,7 +211,9 @@ typedef struct kb_snapshot {
    * Only read for tasks that carry KB_TASK_HAS_PREFERRED_NODE_AFFINITY; all three may be NULL otherwise.  The CPU oracle
    * evaluates them (count = sum of the weights of the matching terms, NormalizeReduce(10) over the feasible nodes);
    * the engine evaluates them in cycle_kernel, and on the per-visit kernels (other record geometries, sessions with inter-pod terms)
-   * with a pass over the feasible nodes before every visit of such a class; refused only on a sharded node axis. */
+   * with a pass over the feasible nodes before every visit of such a class; refused only on a sharded node axis.  preempt orders
+   * its nodes with them too (the max count taken afresh for every preemptor over all nodes that pass the predicates); reclaim
+   * never scores. */
   const uint32_t* task_n_pref_terms;  /* [T] 0..KB_MAX_PREF_TERMS                                    */
   const uint64_t* task_pref_terms;    /* [KB_MAX_PREF_TERMS][W][T] requirement atoms of term p: ALL must hold on the node */
   const int32_t*  task_pref_weights;  /* [KB_MAX_PREF_TERMS][T] PreferredSchedulingTerm.Weight (0 = term skipped) */

@@ -96,8 +96,8 @@ struct ClassRec {
 };
 
 // Preferred node-affinity terms of a class (NodeAffinityPriority, vendor/.../priorities/node_affinity.go:34-77): requirement
-// atoms that must ALL hold on the node + the term's weight.  Evaluated by cycle_kernel (two-pass scan, kb_pipe.cuh) and by
-// the emulation; the per-launch kernels still refuse sessions with preferred terms.
+// atoms that must ALL hold on the node + the term's weight.  Evaluated by cycle_kernel (two-pass scan, kb_pipe.cuh), the
+// per-visit kernels (kb_kernels.cuh), preempt's sweep (kb_evict.h) and the emulation.
 struct ClassPref {
   uint64_t term[KB_MAX_PREF_TERMS][KB_MAX_W];
   int32_t  weight[KB_MAX_PREF_TERMS];

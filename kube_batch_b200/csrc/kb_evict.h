@@ -5,7 +5,8 @@
 // (gang.go:70-94, priority.go:81-100, drf.go:84-110, proportion.go:171-196, conformance.go:41-63).
 //
 // Shape of the work: per PREEMPTOR task one pass over all nodes — ssn.PredicateFn (K1, the same eval_pair as allocate),
-// for preempt also the node score (K2, util.PrioritizeNodes + util.SortNodes == arg-max of the packed key), and per node a
+// for preempt also the node score (K2, util.PrioritizeNodes + util.SortNodes == arg-max of the packed key; a class with preferred
+// node-affinity terms first takes one more pass over all nodes for NodeAffinityPriority's max count), and per node a
 // short SERIAL walk over the node's Running tasks (the plugins' filters are order-dependent: drf / proportion subtract
 // cumulatively) -> "first node in order whose victims cover InitResreq".  The node axis is data-parallel (one thread per
 // node, block arg-max); the commit on the chosen node (evictions, Pipeline, Statement log) is serial.  The control flow
@@ -51,6 +52,8 @@ struct EvictCtl {
   // swept and its class (written by the master thread before it posts the command)
   uint32_t cmd_seq, arrived, n_workers, pad0;
   uint32_t cls_valid, cls_id;      // class record currently in `cls`      // master -> workers: sweep command counter (~0u = exit); workers -> master: CTAs done
+  uint32_t pass;                   // master -> workers: 1 = pass 1 of a preferred node-affinity class (max count), 0 = the sweep
+  uint32_t pmax;                   // workers -> master (pass 1): max count; master -> workers (sweep): the normalisation max
   unsigned long long red;
   Preemptor pre;
   ClassRec cls;
@@ -176,8 +179,32 @@ KB_HD bool evict_is_victim(const DevSession& S, const EvictDev& E, const Preempt
   return v;
 }
 
-// K1 (+K2 for preempt) + the victim walk of one node: packed key (score, node) if the node's victims cover InitResreq, else 0
-KB_HD uint64_t evict_node_key(const DevSession& S, const EvictDev& E, const Preemptor& P, const ClassRec& c, const uint32_t node, uint32_t* err) {
+// The preferred node-affinity terms preempt's node order reads for this preemptor (util.PrioritizeNodes with NodeAffinityPriority,
+// registered by nodeorder; the condition visit_kernel uses), nullptr when the score has no such term.  reclaim walks ssn.Nodes in
+// order and never scores (reclaim.go:113-115).
+KB_HD const ClassPref* evict_pref(const DevSession& S, const Preemptor& P) {
+  return (P.mode != 0 && S.class_pref != nullptr && S.cf.nodeorder && S.class_pref[P.cls].n != 0) ? &S.class_pref[P.cls] : nullptr;
+}
+
+// Pass 1 for such a preemptor, per node: its NodeAffinityPriority count when the node passes ssn.PredicateFn, else 0.
+// NormalizeReduce divides by the max count over util.PredicateNodes (preempt.go:180-189, reduce.go:28-63), i.e. over EVERY node
+// that passes the predicates — also nodes without Running tasks or eligible victims, and full nodes (preempt never checks Idle) —
+// so this runs on all nodes, not only on those evict_node_key gives a key.  The max starts at 0, so 0 stands for "not counted".
+KB_HD uint32_t evict_pref_count(const DevSession& S, const ClassRec& c, const ClassPref& cp, const uint32_t node) {
+  const size_t tile_u64 = (size_t)S.ncols * TILE_NODES;
+  TileAcc acc{S.tiles + (size_t)(node / TILE_NODES) * tile_u64, node % TILE_NODES, S.cf.R, S.cf.W};
+  bool pok = true;
+  (void)eval_pair(S.cf, c, acc, node, nullptr, &pok);
+  if (!pok) return 0;
+  const int32_t cnt = pref_count(cp, acc, S.cf.W);
+  return cnt > 0 ? (uint32_t)cnt : 0u;
+}
+
+// K1 (+K2 for preempt) + the victim walk of one node: packed key (score, node) if the node's victims cover InitResreq, else 0.
+// cp / pmax: evict_pref and the max of evict_pref_count over all nodes (pass 1); the score gains 10 * count / pmax times
+// nodeaffinity.weight (a negative weight is already folded into cf.score_bias).
+KB_HD uint64_t evict_node_key(const DevSession& S, const EvictDev& E, const Preemptor& P, const ClassRec& c, const ClassPref* cp, const uint32_t pmax,
+                              const uint32_t node, uint32_t* err) {
   const uint32_t R = S.cf.R, W = S.cf.W, n = E.n_run;
   const uint32_t lo = E.node_off[node], hi = E.node_off[node + 1];
   if (lo == hi) return 0;
@@ -200,9 +227,9 @@ KB_HD uint64_t evict_node_key(const DevSession& S, const EvictDev& E, const Pree
   }
   if (nv == 0) return 0;                                                   // reclaim.go:141-144 / validateVictims
   if (!res_less_equal(R, [&](uint32_t k) { return c.initreq[k]; }, [&](uint32_t k) { return all[k]; })) return 0;   // :147-154
-  int64_t score = S.cf.score_bias;
-  if (P.mode != 0) score = node_score(S.cf, c, acc);                      // util.SortNodes: best score first, node order among equals
-  return pack_key(score, node);
+  if (P.mode == 0) return pack_key(S.cf.score_bias, node);
+  const uint64_t key = pack_key(node_score(S.cf, c, acc), node);          // util.SortNodes: best score first, node order among equals
+  return cp ? add_pref_term(key, (int64_t)S.w_nodeaff, (int64_t)pref_count(*cp, acc, W), (int64_t)pmax) : key;
 }
 
 // ---- state changes (thread 0) ----
@@ -386,9 +413,13 @@ struct CpuExec {
   KB_HD bool jobs_scanned() const { return false; }
   KB_HD void clear_max() {}
   uint64_t sweep(const DevSession& S, const EvictDev& E, const Preemptor& P, const ClassRec& c) {      // the node axis, serially
+    const ClassPref* cp = evict_pref(S, P);
+    uint32_t pmax = 0;
+    if (cp)                                                       // pass 1 (preferred terms only): the normalisation max, on the current records
+      for (uint32_t n = 0; n < S.N; ++n) { const uint32_t v = evict_pref_count(S, c, *cp, n); pmax = v > pmax ? v : pmax; }
     uint64_t best = 0;
     uint32_t err = 0;
-    for (uint32_t n = 0; n < S.N; ++n) { const uint64_t k = evict_node_key(S, E, P, c, n, &err); best = k > best ? k : best; }
+    for (uint32_t n = 0; n < S.N; ++n) { const uint64_t k = evict_node_key(S, E, P, c, cp, pmax, n, &err); best = k > best ? k : best; }
     if (err) E.ctl->error = err;
     return best;
   }
@@ -472,7 +503,8 @@ KB_HD bool try_preemptor(X& x, const DevSession& S, const EvictDev& E, const uin
   x.sync();
   const Preemptor& P = x.pre();
   const ClassRec& c = x.cls();
-  // An identical sweep (same class, same filter, nothing changed since) that found no node finds none again: skip it.
+  // An identical sweep (same class, same filter, nothing changed since) that found no node finds none again: skip it.  This holds
+  // with preferred node-affinity terms too: their scores only order the valid nodes, whether a valid node exists does not depend on them.
   const uint32_t fkey = mode == 0 ? P.queue : job;
   const bool known_fail = ctl.fail_valid && ctl.fail_cls == P.cls && ctl.fail_mode == mode && ctl.fail_key == fkey && ctl.fail_version == ctl.version;
   uint64_t best = 0;

@@ -9,6 +9,10 @@
 //   worker  CTAs poll the command word (acquire), sweep their share of the nodes — one node per thread per iteration: K1
 //           predicate, K2 score for preempt, the serial victim walk of the node's Running tasks — reduce the packed keys
 //           (warp REDUX, one 64-bit atomicMax per CTA) and arrive.
+//   pass 1  a preempting class with preferred node-affinity terms (evict_pref) takes one more round trip through the same mailbox
+//           before its sweep: the workers reduce the NodeAffinityPriority max count over all their nodes (warp REDUX.MAX, one
+//           atomicMax per CTA into EvictCtl.pmax) and arrive; the sweep command that follows reads pmax from the mailbox.  Workers
+//           keep the class's ClassPref in shared memory and copy it only when the class changes.
 //
 // Coherence: the master mutates node records, job / queue accounting and the Running tasks' states between two sweeps.  It
 // publishes them with a release store of the command word; thread 0 of every worker CTA reads that word with ld.acquire.gpu —
@@ -44,14 +48,21 @@ struct MasterExec {
   __device__ __forceinline__ void clear_max() {}
   __device__ __forceinline__ ClassRec& cls() { return g->cls; }
   __device__ __forceinline__ Preemptor& pre() { return g->pre; }
-  __device__ __forceinline__ uint64_t sweep(const DevSession&, const EvictDev&, const Preemptor&, const ClassRec&) {
-    g->red = 0ull;
+  __device__ __forceinline__ void post(const uint32_t pass) {     // one command to every worker CTA, back when all have arrived
+    g->pass = pass;
     g->arrived = 0u;
-    __threadfence();                                 // the mailbox (pre, cls) and every table write of earlier commits are visible first
+    __threadfence();                                 // the mailbox (pre, cls, pmax) and every table write of earlier commits are visible first
     seq += 1;
     ev_st_release(&g->cmd_seq, seq);
     const uint32_t nw = g->n_workers;
     while (ev_ld_acquire(&g->arrived) < nw) __nanosleep(40);
+  }
+  __device__ __forceinline__ uint64_t sweep(const DevSession& S, const EvictDev&, const Preemptor& P, const ClassRec&) {
+    // preferred node-affinity terms: pass 1 leaves the max count in g->pmax, which is then the sweep's normalisation.  It is
+    // taken afresh for every sweep: a Pipeline raises a node's pod count, and max_pods can drop that node together with its count.
+    if (evict_pref(S, P)) { g->pmax = 0u; post(1u); }
+    g->red = 0ull;
+    post(0u);
     return *((volatile unsigned long long*)&g->red);
   }
 };
@@ -73,16 +84,19 @@ evict_kernel(const __grid_constant__ DevSession S, const __grid_constant__ Evict
   // ---------------- workers ----------------
   __shared__ ClassRec s_cls;
   __shared__ Preemptor s_pre;
+  __shared__ ClassPref s_pref;                     // preferred node-affinity terms of class s_pref_cls
   __shared__ uint64_t s_red[EVICT_THREADS / 32];
-  __shared__ uint32_t s_cmd, s_err;
+  __shared__ uint32_t s_cmd, s_err, s_pass, s_pmax, s_pref_cls;
   const uint32_t nw = gridDim.x - 1;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   uint32_t seen = 0;
+  if (threadIdx.x == 0) s_pref_cls = 0xFFFFFFFFu;
   for (;;) {
     if (threadIdx.x == 0) {
       uint32_t v;
       while ((v = ev_ld_acquire(&g->cmd_seq)) == seen) __nanosleep(40);
       s_cmd = v; s_err = 0;
+      s_pass = *((volatile uint32_t*)&g->pass); s_pmax = *((volatile uint32_t*)&g->pmax);
     }
     __syncthreads();
     const uint32_t cmd = s_cmd;
@@ -97,10 +111,40 @@ evict_kernel(const __grid_constant__ DevSession S, const __grid_constant__ Evict
       for (uint32_t i = threadIdx.x; i < sizeof(Preemptor) / 4; i += EVICT_THREADS) pd[i] = ps[i];
     }
     __syncthreads();
+    const ClassPref* cp = evict_pref(S, s_pre);    // uniform across the CTA
+    if (cp && s_pref_cls != s_pre.cls) {           // 160 B, only when the class changes
+      const uint32_t* src = reinterpret_cast<const uint32_t*>(cp);
+      uint32_t* dst = reinterpret_cast<uint32_t*>(&s_pref);
+      for (uint32_t i = threadIdx.x; i < sizeof(ClassPref) / 4; i += EVICT_THREADS) dst[i] = src[i];
+      __syncthreads();
+      if (threadIdx.x == 0) s_pref_cls = s_pre.cls;
+    }
+    if (s_pass == 1u) {                            // pass 1: max NodeAffinityPriority count over this CTA's nodes
+      uint32_t m = 0;
+      for (uint32_t n = blockIdx.x * EVICT_THREADS + threadIdx.x; n < S.N; n += nw * EVICT_THREADS) {
+        const uint32_t v = evict_pref_count(S, s_cls, s_pref, n);
+        m = v > m ? v : m;
+      }
+      m = __reduce_max_sync(0xFFFFFFFFu, m);
+      if (lane == 0) s_red[warp] = m;
+      __syncthreads();
+      if (warp == 0) {
+        const uint32_t x = __reduce_max_sync(0xFFFFFFFFu, lane < EVICT_THREADS / 32 ? (uint32_t)s_red[lane] : 0u);
+        if (lane == 0) {
+          if (x) atomicMax(&g->pmax, x);
+          __threadfence();
+          atomicAdd(&g->arrived, 1u);
+        }
+      }
+      __syncthreads();
+      continue;
+    }
     uint64_t best = 0;
     uint32_t err = 0;
+    const ClassPref* scp = cp ? &s_pref : nullptr;
+    const uint32_t pmax = s_pmax;
     for (uint32_t n = blockIdx.x * EVICT_THREADS + threadIdx.x; n < S.N; n += nw * EVICT_THREADS) {
-      const uint64_t k = evict_node_key(S, E, s_pre, s_cls, n, &err);
+      const uint64_t k = evict_node_key(S, E, s_pre, s_cls, scp, pmax, n, &err);
       best = k > best ? k : best;
     }
     if (err) s_err = err;

@@ -296,6 +296,31 @@ def add_host_spread(s: Snapshot, frac: float = 0.1, labels: int = 8, seed: int =
     return s
 
 
+def add_node_pref(s: Snapshot, frac: float = 0.3, seed: int = 11) -> Snapshot:
+    """Gives `frac` of the PodGroups the preferred zone affinity Helm charts and operators commonly set: every pod of the group carries
+    1-3 nodeAffinity.preferredDuringSchedulingIgnoredDuringExecution terms {zone In [z]} with weights from {1, 10, 50, 100}.  The zones
+    are the label atoms `generate` sets (word 0, bits 0-2).  Fills KB_TASK_HAS_PREFERRED_NODE_AFFINITY and task_n_pref_terms /
+    task_pref_terms / task_pref_weights exactly as builder.flatten would for such pods."""
+    rng = np.random.Generator(np.random.PCG64(seed))
+    for j in range(s.J):
+        lo, hi = int(s.job_task_off[j]), int(s.job_task_off[j + 1])
+        if hi == lo or rng.random() >= frac:
+            continue
+        nt = int(rng.integers(1, 4))
+        zones = rng.integers(0, 3, size=nt)
+        weights = rng.choice([1, 10, 50, 100], size=nt)
+        s.task_flags[lo:hi] |= abi.KB_TASK_HAS_PREFERRED_NODE_AFFINITY
+        s.task_n_pref_terms[lo:hi] = nt
+        s.task_pref_terms[:, :, lo:hi] = 0
+        s.task_pref_weights[:, lo:hi] = 0
+        for p in range(nt):
+            s.task_pref_terms[p, 0, lo:hi] = np.uint64(1) << np.uint64(zones[p])
+            s.task_pref_weights[p, lo:hi] = weights[p]
+    s.meta["pref_tasks"] = int((s.task_n_pref_terms != 0).sum())
+    s.invalidate()
+    return s
+
+
 # ------------------------------------------------------------------------------------------------
 # small randomised sessions for property / parity tests: every feature of the path at once
 # ------------------------------------------------------------------------------------------------

@@ -1,5 +1,6 @@
 """Time kb_cycle (the shipped action list on ONE session) on a BASELINE config + its Running filler pods, and check it against
-the oracle.   python tools/cycle_time.py c3 [preemptable_frac] [oracle:0|1]"""
+the oracle.   python tools/cycle_time.py c3 [preemptable_frac] [oracle:0|1] [node_pref_frac]
+node_pref_frac > 0: that share of the PodGroups carries preferred zone affinity (synth.add_node_pref)."""
 import sys, os, time, json
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
@@ -8,13 +9,18 @@ from kube_batch_b200 import engine, synth, digest
 name = sys.argv[1] if len(sys.argv) > 1 else "c3"
 frac = float(sys.argv[2]) if len(sys.argv) > 2 else 0.3
 with_oracle = int(sys.argv[3]) if len(sys.argv) > 3 else 1
+pref_frac = float(sys.argv[4]) if len(sys.argv) > 4 else 0.0
 acts = ("reclaim", "allocate", "backfill", "preempt")
 snap, conf = synth.make(name)
+if pref_frac > 0:
+    synth.add_node_pref(snap, pref_frac)
 run = synth.running_of(snap, frac)
 eng = engine.Engine(0)
 t0 = time.time(); eng.load(snap, conf).load_running(run); t1 = time.time()
-out = {"workload": f"{name}: {snap.T} pending tasks / {snap.N} nodes / {len(run['node'])} Running pods one by one, {frac:.0%} of the filler PodGroups preemptable",
-       "actions": list(acts), "load_ms": 1e3 * (t1 - t0)}
+workload = f"{name}: {snap.T} pending tasks / {snap.N} nodes / {len(run['node'])} Running pods one by one, {frac:.0%} of the filler PodGroups preemptable"
+if pref_frac > 0:
+    workload += f", {pref_frac:.0%} of the PodGroups with preferred zone affinity ({snap.meta['pref_tasks']} tasks)"
+out = {"workload": workload, "actions": list(acts), "load_ms": 1e3 * (t1 - t0)}
 for rep in range(3):
     t0 = time.time(); res, ev, order, bounds = eng.cycle(acts); t1 = time.time()
     st = res.stats
