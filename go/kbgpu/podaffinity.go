@@ -34,7 +34,8 @@ type podAff struct {
 	keysetDomains             []uint32
 	groupKeyset               []uint32
 	groupCount0, groupTotal0  []int32
-	taskForbid, taskContrib   []uint64
+	taskForbid, taskContrib   []uint64 // groups 0..63
+	taskXgroupOff, taskXgroup []uint32 // groups >= 64: (g << 2) | KB_XGROUP_FORBID | KB_XGROUP_CONTRIB; nil when nGroups <= 64
 	taskNeed, taskKind        []int32
 	nodeKindCount0            []int32 // [nKinds][N]
 	kindUnbound               []uint8
@@ -277,7 +278,13 @@ func flattenPodAffinity(ssn *framework.Session, f *Flat, nidx map[string]int, sn
 		groups = append(groups, group{keyset, m})
 		return g
 	}
-	forbid := map[int]uint64{}
+	forbid := map[int]map[int]bool{} // pending type -> the groups it forbids (any number of groups)
+	addForbid := func(ty, g int) {
+		if forbid[ty] == nil {
+			forbid[ty] = map[int]bool{}
+		}
+		forbid[ty][g] = true
+	}
 	need := map[int]int32{}
 	selfMatch := map[int]bool{}
 	for _, ty := range pendTypes {
@@ -334,7 +341,7 @@ func flattenPodAffinity(ssn *framework.Session, f *Flat, nidx map[string]int, sn
 				return false
 			})
 			for _, ty := range victims {
-				forbid[ty] |= 1 << uint(g)
+				addForbid(ty, g)
 			}
 		}
 	}
@@ -372,15 +379,18 @@ func flattenPodAffinity(ssn *framework.Session, f *Flat, nidx map[string]int, sn
 			}
 			g := addGroup(fmt.Sprintf("B|%s|%d", strings.Join(pkeys, "\x01"), ks), ks, all)
 			if anti {
-				forbid[ty] |= 1 << uint(g)
+				addForbid(ty, g)
 			} else {
 				need[ty] = int32(g)
 				selfMatch[ty] = all(pod) // targetPodMatchesAffinityOfPod(pod, pod)
 			}
 		}
 	}
-	if len(groups) > int(C.KB_MAX_AFF_GROUPS) || len(keysetID) > 64 {
-		return nil, &ErrUnsupported{fmt.Sprintf("%d inter-pod affinity counter groups / %d key sets: more than 64", len(groups), len(keysetID))}
+	if len(groups) > int(C.KB_MAX_AFF_GROUPS) {
+		return nil, &ErrUnsupported{fmt.Sprintf("%d inter-pod affinity counter groups: more than %d", len(groups), int(C.KB_MAX_AFF_GROUPS))}
+	}
+	if len(keysetID) > 64 {
+		return nil, &ErrUnsupported{fmt.Sprintf("%d topology key sets: more than 64", len(keysetID))}
 	}
 	pa.nGroups = len(groups)
 	gOff := make([]int, len(groups)+1)
@@ -528,15 +538,37 @@ func flattenPodAffinity(ssn *framework.Session, f *Flat, nidx map[string]int, sn
 	pa.taskForbid, pa.taskContrib = make([]uint64, max1(T)), make([]uint64, max1(T))
 	pa.taskNeed, pa.taskKind = make([]int32, max1(T)), make([]int32, max1(T))
 	pa.taskWeightOff = make([]uint32, T+1)
+	if len(groups) > 64 {
+		pa.taskXgroupOff = make([]uint32, T+1)
+	}
 	for t := 0; t < T; t++ {
 		ty := ptype[t]
-		pa.taskForbid[t] = forbid[ty]
 		pa.taskNeed[t] = need[ty]
 		pa.taskKind[t] = pkind[ty]
-		for g, gr := range groups {
-			if gr.member[ty] {
-				pa.taskContrib[t] |= 1 << uint(g)
+		for g, gr := range groups { // groups < 64: bits of the masks; the others: entries of task_xgroup, ascending
+			f, c := forbid[ty][g], gr.member[ty]
+			if g < 64 {
+				if f {
+					pa.taskForbid[t] |= 1 << uint(g)
+				}
+				if c {
+					pa.taskContrib[t] |= 1 << uint(g)
+				}
+				continue
 			}
+			if f || c {
+				e := uint32(g) << 2
+				if f {
+					e |= C.KB_XGROUP_FORBID
+				}
+				if c {
+					e |= C.KB_XGROUP_CONTRIB
+				}
+				pa.taskXgroup = append(pa.taskXgroup, e)
+			}
+		}
+		if pa.taskXgroupOff != nil {
+			pa.taskXgroupOff[t+1] = uint32(len(pa.taskXgroup))
 		}
 		for _, e := range wlist[ty] {
 			pa.weightKind = append(pa.weightKind, e.kind)
@@ -591,5 +623,8 @@ func (pa *podAff) cPodAffinity(a *arena) *C.kb_pod_affinity {
 	c.kind_unbound = (*C.uint8_t)(a.put(unsafe.Pointer(&ku[0]), uintptr(len(ku))))
 	c.task_weight_off = u32(pa.taskWeightOff)
 	c.weight_kind, c.weight_keyset, c.weight_value = i32(pa.weightKind), i32(pa.weightKeyset), i64(pa.weightValue)
+	if pa.taskXgroupOff != nil { // NULL for sessions with at most 64 groups
+		c.task_xgroup_off, c.task_xgroup = u32(pa.taskXgroupOff), u32(pa.taskXgroup)
+	}
 	return (*C.kb_pod_affinity)(a.put(unsafe.Pointer(&c), unsafe.Sizeof(c)))
 }

@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define KB_ABI_VERSION 1u
+#define KB_ABI_VERSION 2u
 
 /* Compile-time capacity of the dense encodings. */
 #define KB_MAX_R 8          /* resource dims: 0 = cpu (milli), 1 = memory (bytes), 2.. = scalar resources (milli) */
@@ -113,11 +113,19 @@ typedef enum kb_status {
  *      49-63) returns the first node it finds holding ANY such pod — a Go map iteration; deterministic rule (SURVEY.md 8c):
  *      the lowest node index holding one (`first_unbound_node`, kept current by the engine).
  *      score = int(10 * (count - min) / (max - min)) over the feasible nodes, min and max starting at 0.
+ *
+ * A session may have up to KB_MAX_AFF_GROUPS counter groups.  A task names groups 0..63 in the masks task_forbid /
+ * task_contrib (bit g = group g) and groups 64 and above in the extension list task_xgroup (entries task_xgroup_off[t] ..
+ * task_xgroup_off[t+1]-1, each (g << 2) | KB_XGROUP_FORBID | KB_XGROUP_CONTRIB, g >= 64, at least one of the two bits set).
+ * Both lists may be NULL when n_groups <= 64.  Sessions with 64 groups or fewer carry empty lists and take the same path they
+ * take without them.  Key sets stay <= 64 (a class's weight key sets are a mask).
  */
-#define KB_MAX_AFF_GROUPS 64
+#define KB_MAX_AFF_GROUPS 4096
+#define KB_XGROUP_FORBID  1u      /* task_xgroup: a member of the group in the node's domain rejects the node for this task */
+#define KB_XGROUP_CONTRIB 2u      /* task_xgroup: the task becomes a member of the group once it is Allocated               */
 typedef struct kb_pod_affinity {
   uint32_t n_keysets;             /* distinct topology key sets                                                              */
-  uint32_t n_groups;              /* <= KB_MAX_AFF_GROUPS                                                                     */
+  uint32_t n_groups;              /* <= KB_MAX_AFF_GROUPS (more -> KB_E_UNSUPPORTED_FEATURE)                                  */
   uint32_t n_kinds;
   uint32_t n_weights;
   int32_t  first_unbound_node;    /* -1: no pod with an empty Spec.NodeName sits on a node at session open                    */
@@ -137,6 +145,8 @@ typedef struct kb_pod_affinity {
   const int32_t*  weight_kind;    /* [n_weights]                                                                              */
   const int32_t*  weight_keyset;  /* [n_weights] a single-key key set                                                         */
   const int64_t*  weight_value;   /* [n_weights]                                                                              */
+  const uint32_t* task_xgroup_off;/* [T+1] the task's entries in task_xgroup; NULL allowed when n_groups <= 64                */
+  const uint32_t* task_xgroup;    /* (g << 2) | KB_XGROUP_FORBID | KB_XGROUP_CONTRIB for the groups g >= 64 the task names     */
 } kb_pod_affinity;
 
 /*

@@ -14,7 +14,7 @@ KB_ENGINE_CHAIN2 = 1 << 3
 KB_ENGINE_CHAIN4 = 1 << 4
 KB_ENGINE_NO_PIPE = 1 << 5
 KB_ENGINE_SHARD = 1 << 6
-KB_ABI_VERSION = 1
+KB_ABI_VERSION = 2
 KB_MAX_R = 8
 KB_MAX_W = 4
 KB_MAX_AFF_TERMS = 4
@@ -42,7 +42,9 @@ KB_SNAPSHOT_PLACED_POD_AFFINITY = 1 << 0
 KB_SNAPSHOT_LISTED_POD_WITHOUT_NODE = 1 << 1
 KB_TASK_HAS_PREFERRED_NODE_AFFINITY = 1 << 2
 KB_TASK_AFF_SELF_MATCH = 1 << 3
-KB_MAX_AFF_GROUPS = 64
+KB_MAX_AFF_GROUPS = 4096
+KB_XGROUP_FORBID = 1
+KB_XGROUP_CONTRIB = 2
 
 KB_KIND_NONE = 0
 KB_KIND_ALLOCATED = 1
@@ -121,6 +123,11 @@ POD_AFFINITY_ARRAYS = [
     ("weight_keyset", C.c_int32, "i4"),
     ("weight_value", C.c_int64, "i8"),
 ]
+# groups >= 64 (include/kbgpu.h): optional, NULL when the dict has no such key (sessions with at most 64 groups)
+POD_AFFINITY_XARRAYS = [
+    ("task_xgroup_off", C.c_uint32, "u4"),
+    ("task_xgroup", C.c_uint32, "u4"),
+]
 
 
 class kb_pod_affinity(C.Structure):
@@ -132,7 +139,7 @@ class kb_pod_affinity(C.Structure):
         ("n_weights", C.c_uint32),
         ("first_unbound_node", C.c_int32),
         ("reserved", C.c_uint32),
-    ] + [(name, C.POINTER(ct)) for name, ct, _ in POD_AFFINITY_ARRAYS]
+    ] + [(name, C.POINTER(ct)) for name, ct, _ in POD_AFFINITY_ARRAYS + POD_AFFINITY_XARRAYS]
 
 
 def pod_affinity_to_c(pa):
@@ -143,6 +150,14 @@ def pod_affinity_to_c(pa):
     r.n_weights = int(pa["n_weights"]); r.first_unbound_node = int(pa["first_unbound_node"])
     keep = []
     for name, ct, dt in POD_AFFINITY_ARRAYS:
+        a = np.ascontiguousarray(pa[name], dtype=np.dtype(dt)).reshape(-1)
+        if a.size == 0:
+            a = np.zeros(1, dtype=np.dtype(dt))
+        keep.append(a)
+        setattr(r, name, a.ctypes.data_as(C.POINTER(ct)))
+    for name, ct, dt in POD_AFFINITY_XARRAYS:
+        if pa.get(name) is None:
+            continue
         a = np.ascontiguousarray(pa[name], dtype=np.dtype(dt)).reshape(-1)
         if a.size == 0:
             a = np.zeros(1, dtype=np.dtype(dt))

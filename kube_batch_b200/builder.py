@@ -644,8 +644,7 @@ def flatten_pod_affinity(nodes, pending, existing, s, on_node, status_of, in_ses
             else:
                 need_ty[ty] = g
                 self_ty[ty] = all(_props_match(p, pr) for pr in props)      # targetPodMatchesAffinityOfPod(pod, pod)
-    NG = len(groups)
-    assert NG <= abi.KB_MAX_AFF_GROUPS, "more than 64 inter-pod affinity counter groups"
+    NG = len(groups)          # forbid_ty / contrib_ty are bit sets over all NG groups: bits 0..63 go to the masks, the rest to task_xgroup
     g_off = np.zeros(NG + 1, dtype=np.int64)
     for g in range(NG):
         g_off[g + 1] = g_off[g] + dom_count[g_keyset[g]]
@@ -740,6 +739,13 @@ def flatten_pod_affinity(nodes, pending, existing, s, on_node, status_of, in_ses
     if any(p.pod_affinity is not None or p.pod_anti_affinity is not None for p in existing):
         s.flags = int(getattr(s, "flags", 0)) | abi.KB_SNAPSHOT_PLACED_POD_AFFINITY
 
+    M64 = (1 << 64) - 1
+
+    def xgroups(ty):
+        f, c = forbid_ty[ty] >> 64, contrib_ty[ty] >> 64
+        return [((64 + i) << 2) | ((f >> i) & 1) * abi.KB_XGROUP_FORBID | ((c >> i) & 1) * abi.KB_XGROUP_CONTRIB
+                for i in range(max(f.bit_length(), c.bit_length())) if ((f | c) >> i) & 1]
+
     NKS = len(keysets)
     pa = {
         "n_keysets": NKS, "n_groups": NG, "n_kinds": NK, "n_weights": len(wk), "first_unbound_node": -1,
@@ -748,9 +754,9 @@ def flatten_pod_affinity(nodes, pending, existing, s, on_node, status_of, in_ses
         "group_keyset": np.array(g_keyset if NG else [0], dtype=np.uint32),
         "group_count0": count0 if count0.size else np.zeros(1, dtype=np.int32),
         "group_total0": total0 if NG else np.zeros(1, dtype=np.int32),
-        "task_forbid": np.array([forbid_ty[ty] for ty in ptype] or [0], dtype=np.uint64),
+        "task_forbid": np.array([forbid_ty[ty] & M64 for ty in ptype] or [0], dtype=np.uint64),
         "task_need": np.array([need_ty[ty] for ty in ptype] or [-1], dtype=np.int32),
-        "task_contrib": np.array([contrib_ty[ty] for ty in ptype] or [0], dtype=np.uint64),
+        "task_contrib": np.array([contrib_ty[ty] & M64 for ty in ptype] or [0], dtype=np.uint64),
         "task_kind": np.array([pkind_ty[ty] for ty in ptype] or [-1], dtype=np.int32),
         "node_kind_count0": kc0,
         "kind_unbound": np.array(kind_unbound or [0], dtype=np.uint8),
@@ -759,6 +765,10 @@ def flatten_pod_affinity(nodes, pending, existing, s, on_node, status_of, in_ses
         "weight_keyset": np.array(wks or [0], dtype=np.int32),
         "weight_value": np.array(wv or [0], dtype=np.int64),
     }
+    if NG > 64:               # groups >= 64: per task the entries (g << 2) | KB_XGROUP_FORBID | KB_XGROUP_CONTRIB
+        xl = [xgroups(ty) for ty in ptype]
+        pa["task_xgroup_off"] = np.concatenate([[0], np.cumsum([len(x) for x in xl], dtype=np.int64)]).astype(np.uint32)
+        pa["task_xgroup"] = np.array([e for x in xl for e in x] or [0], dtype=np.uint32)
 
     # ---- the raw objects (what a checker that walks the pods one by one needs): pending pods in task order, then the others ----
     lset, tset = set(id(p) for p in listed), set(id(p) for p in in_tasks)

@@ -33,9 +33,16 @@
 
 namespace kb {
 
+// A forbidden counter group >= 64 of a class, resolved by the host build so that the scan goes node_domain -> cnt directly.
+struct AffX {
+  uint32_t row;           // group_keyset[g] * N: the key set's row of node_domain
+  uint32_t off;           // group_off[g]: the group's counters
+};
+
+// Groups 0..63 are bits of the masks; groups >= 64 (kb_pod_affinity.task_xgroup) sit in two packed per-class lists.
 struct ClassAff {
-  uint64_t forbid;        // groups whose members in the node's domain reject the node
-  uint64_t contrib;       // groups the task joins once Allocated
+  uint64_t forbid;        // groups < 64 whose members in the node's domain reject the node
+  uint64_t contrib;       // groups < 64 the task joins once Allocated
   uint64_t w_keysets;     // key sets that appear in the class's weight list
   int32_t  need;          // group the required pod-affinity terms need, -1 none
   int32_t  kind;          // kind of the placed pod, -1 none
@@ -45,6 +52,10 @@ struct ClassAff {
   uint32_t pred_multi_ok; // the predicate part of the class survives its OWN placements: the only counters it both joins and reads
                           // belong to key sets whose domains are single nodes (kubernetes.io/hostname), so a placement changes
                           // nothing but the chosen node — the candidate list stays exact and a run may place several tasks
+  uint32_t xf_off, xf_cnt;  // forbidden groups >= 64: AffDev.xf[xf_off .. xf_off + xf_cnt); the first xs_cnt of them are also joined
+  uint32_t xs_cnt;          //   (the groups aff_self_blocks reads)
+  uint32_t xc_off, xc_cnt;  // joined groups >= 64: AffDev.xc[xc_off .. xc_off + xc_cnt) (group ids)
+  uint32_t x_pad;
 };
 
 struct AffDev {
@@ -55,11 +66,14 @@ struct AffDev {
   uint32_t dom_total;             // sum of the key sets' domain counts (size of dom_sum)
   uint32_t has_pref;              // some class carries preferred NODE-affinity terms and the session runs on the per-visit kernels:
                                   // pass 2 also reduces the max count over the feasible nodes (NodeAffinityPriority, minmax[2])
+  uint32_t has_x;                 // some class names groups >= 64 (xf / xc lists): sessions without skip every list walk
   const int32_t*  node_domain;    // [n_keysets][N]
   const uint32_t* keyset_off;     // [n_keysets + 1] offsets into dom_sum
   const uint32_t* group_keyset;   // [n_groups]
   const uint32_t* group_off;      // [n_groups] offsets into cnt
   const ClassAff* cls;            // [C]
+  const AffX*     xf;             // the classes' forbidden groups >= 64, packed (ClassAff.xf_off)
+  const uint32_t* xc;             // the classes' joined groups >= 64, packed (ClassAff.xc_off)
   const int32_t*  w_kind;
   const int32_t*  w_keyset;
   const int64_t*  w_value;
@@ -76,7 +90,7 @@ struct AffDev {
 // placement changes beyond the chosen node: a weight list (allocate view: nodeorder on), or predicate groups over multi-node domains.
 KB_HD bool aff_stop_each(const ClassAff& ca, const bool nodeorder) {
   if (ca.w_cnt != 0 && nodeorder) return true;
-  if (ca.forbid == 0 && ca.need < 0) return false;
+  if (ca.forbid == 0 && ca.xf_cnt == 0 && ca.need < 0) return false;
   return ca.pred_multi_ok == 0;
 }
 
@@ -91,7 +105,10 @@ KB_HD uint32_t aff_lowest_bit(const uint64_t m) {
 // predicate step 10 for a pod of class `ca` on node n (the predicates plugin must be enabled; the caller checks).
 // The counter reads of up to four groups are issued together: each is a chain node_domain -> cnt (an L2 round trip each), and a
 // lone thread only overlaps what it has in flight at once (a class forbidden by 35 groups would cost 35 serial round trips).
-KB_HD bool aff_pred(const AffDev& A, const ClassAff& ca, const uint32_t N, const uint32_t n) {
+// Groups >= 64 come from the class's forbidden list: its first `ns` entries from `xs` (the scan stages them in shared memory),
+// the rest from A.xf.
+KB_HD bool aff_pred(const AffDev& A, const ClassAff& ca, const uint32_t N, const uint32_t n, const AffX* xs = nullptr,
+                    const uint32_t ns = 0) {
   bool ok = true;
   uint64_t f = ca.forbid;
   while (f) {                                    // satisfiesExistingPodsAntiAffinity (:1400-1439) + the pod's own anti-affinity (:1526-1533)
@@ -116,6 +133,28 @@ KB_HD bool aff_pred(const AffDev& A, const ClassAff& ca, const uint32_t N, const
     for (int k = 0; k < 4; ++k) v[k] = d[k] >= 0 ? KB_LDM(&A.cnt[off[k] + (uint32_t)d[k]]) : 0;
     ok = ok && ((v[0] | v[1] | v[2] | v[3]) <= 0);          // counters are never negative
   }
+  for (uint32_t i = 0; A.has_x && i < ca.xf_cnt; i += 4) {   // the same for the groups >= 64
+    int32_t d[4];
+    uint32_t off[4];
+#if defined(__CUDA_ARCH__)
+#pragma unroll
+#endif
+    for (int k = 0; k < 4; ++k) {
+      d[k] = -1; off[k] = 0;
+      const uint32_t j = i + (uint32_t)k;
+      if (j < ca.xf_cnt) {
+        const AffX x = j < ns ? xs[j] : A.xf[ca.xf_off + j];
+        d[k] = A.node_domain[(size_t)x.row + n];
+        off[k] = x.off;
+      }
+    }
+    int32_t v[4];
+#if defined(__CUDA_ARCH__)
+#pragma unroll
+#endif
+    for (int k = 0; k < 4; ++k) v[k] = d[k] >= 0 ? KB_LDM(&A.cnt[off[k] + (uint32_t)d[k]]) : 0;
+    ok = ok && ((v[0] | v[1] | v[2] | v[3]) <= 0);
+  }
   if (ca.need >= 0) {                            // the pod's required affinity terms (:1516-1560)
     const uint32_t g = (uint32_t)ca.need;
     const int32_t d = A.node_domain[(size_t)A.group_keyset[g] * N + n];
@@ -135,6 +174,9 @@ KB_HD bool aff_self_blocks(const AffDev& A, const ClassAff& ca, const uint32_t N
     m &= m - 1;
     if (A.node_domain[(size_t)A.group_keyset[g] * N + n] >= 0) return true;
   }
+  const uint32_t xs = (A.has_x && ca.self_block) ? ca.xs_cnt : 0u;
+  for (uint32_t i = 0; i < xs; ++i)
+    if (A.node_domain[(size_t)A.xf[ca.xf_off + i].row + n] >= 0) return true;
   return false;
 }
 
@@ -185,6 +227,12 @@ KB_HD void aff_commit(const AffDev& A, const ClassAff& ca, const uint32_t N, con
     while (c) {
       const uint32_t g = aff_lowest_bit(c);
       c &= c - 1;
+      A.total[g] = KB_LDM(&A.total[g]) + 1;
+      const int32_t d = A.node_domain[(size_t)A.group_keyset[g] * N + n];
+      if (d >= 0) A.cnt[A.group_off[g] + (uint32_t)d] = KB_LDM(&A.cnt[A.group_off[g] + (uint32_t)d]) + 1;
+    }
+    for (uint32_t i = 0; A.has_x && i < ca.xc_cnt; ++i) {
+      const uint32_t g = A.xc[ca.xc_off + i];
       A.total[g] = KB_LDM(&A.total[g]) + 1;
       const int32_t d = A.node_domain[(size_t)A.group_keyset[g] * N + n];
       if (d >= 0) A.cnt[A.group_off[g] + (uint32_t)d] = KB_LDM(&A.cnt[A.group_off[g] + (uint32_t)d]) + 1;

@@ -218,7 +218,8 @@ struct OffMut { size_t tiles, used, job_pos, job_ready, job_alloc, job_share, jo
                 bf_job_pos, bf_ctl, pipe_g, modlog, pcand, ppref, aff_cnt, aff_total, aff_kind_count, aff_first_unbound, aff_dom_sum, aff_minmax; };
 struct OffImm { size_t classes, ord_task, ord_class, ord_run, ord_peek, job_ord_off, job_min, job_queue, job_prio, job_tb, q_static, q_static_off, q_des, q_des_p, q_ctime, task_class, job_ready0,
                 bf_ord_task, bf_ord_class, bf_ord_run, bf_ord_peek, bf_job_ord_off, bf_jobs, bf_jobs_off, bf_classes, ord_chain, class_pref,
-                aff_node_domain, aff_keyset_off, aff_group_keyset, aff_group_off, aff_cls, aff_w_kind, aff_w_keyset, aff_w_value, aff_kind_unbound; };
+                aff_node_domain, aff_keyset_off, aff_group_keyset, aff_group_off, aff_cls, aff_w_kind, aff_w_keyset, aff_w_value, aff_kind_unbound,
+                aff_xf, aff_xc; };
 
 struct BuiltSession {
   Slab mut, imm;
@@ -293,6 +294,7 @@ struct BuiltSession {
       D.aff.node_domain = (const int32_t*)(ib + oi.aff_node_domain); D.aff.keyset_off = (const uint32_t*)(ib + oi.aff_keyset_off);
       D.aff.group_keyset = (const uint32_t*)(ib + oi.aff_group_keyset); D.aff.group_off = (const uint32_t*)(ib + oi.aff_group_off);
       D.aff.cls = (const ClassAff*)(ib + oi.aff_cls);
+      D.aff.xf = (const AffX*)(ib + oi.aff_xf); D.aff.xc = (const uint32_t*)(ib + oi.aff_xc);
       D.aff.w_kind = (const int32_t*)(ib + oi.aff_w_kind); D.aff.w_keyset = (const int32_t*)(ib + oi.aff_w_keyset);
       D.aff.w_value = (const int64_t*)(ib + oi.aff_w_value); D.aff.kind_unbound = (const uint8_t*)(ib + oi.aff_kind_unbound);
       D.aff.cnt = (int32_t*)(mb + om.aff_cnt); D.aff.total = (int32_t*)(mb + om.aff_total);
@@ -323,8 +325,9 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
   if ((s->flags & KB_SNAPSHOT_PLACED_POD_AFFINITY) && !pa)
     return bfail(e, KB_E_UNSUPPORTED_FEATURE, "a placed pod carries inter-pod (anti)affinity terms: the reference lets it reject nodes for other pods "
                  "(predicates.go:1261-1288); the flattener must hand over kb_snapshot.pod_affinity (no CPU fallback)");
-  if (pa && (pa->n_groups > KB_MAX_AFF_GROUPS || pa->n_keysets > 64))
-    return bfail(e, KB_E_UNSUPPORTED_FEATURE, "kb_pod_affinity: more than 64 counter groups / key sets");
+  if (pa && pa->n_groups > KB_MAX_AFF_GROUPS)
+    return bfail(e, KB_E_UNSUPPORTED_FEATURE, "kb_pod_affinity: %u counter groups, more than %u", pa->n_groups, (unsigned)KB_MAX_AFF_GROUPS);
+  if (pa && pa->n_keysets > 64) return bfail(e, KB_E_UNSUPPORTED_FEATURE, "kb_pod_affinity: more than 64 key sets");
   if (s->flags & ~(KB_SNAPSHOT_PLACED_POD_AFFINITY | KB_SNAPSHOT_LISTED_POD_WITHOUT_NODE)) return bfail(e, KB_E_BADARG, "unknown kb_snapshot.flags bits 0x%x", s->flags);
   if (s->R < 2 || s->R > KB_MAX_R || s->W < 1 || s->W > KB_MAX_W) return bfail(e, KB_E_BADARG, "R=%u / W=%u out of range", s->R, s->W);
   if (s->Q > KB_MAX_Q) return bfail(e, KB_E_BADARG, "Q=%u > KB_MAX_Q", s->Q);
@@ -349,25 +352,56 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
   std::vector<uint64_t> node_aff_bits;                  // [W][N] initial member bits
   std::vector<uint32_t> aff_group_off0;
   bool aff_as_atoms = false;
+  // groups >= 64 of task t: the entries task_xgroup[xg_lo(t) .. xg_hi(t)), (g << 2) | KB_XGROUP_FORBID | KB_XGROUP_CONTRIB
+  const uint32_t* xg_off = pa ? pa->task_xgroup_off : nullptr;
+  const uint32_t* xg_ent = pa ? pa->task_xgroup : nullptr;
+  auto xg_at = [&](uint32_t t, uint32_t i) { return xg_ent[xg_off[t] + i]; };
+  auto xg_lo = [&](uint32_t t) { return xg_off ? xg_off[t] : 0u; };
+  auto xg_hi = [&](uint32_t t) { return xg_off ? xg_off[t + 1] : 0u; };
+  auto xg_same = [&](uint32_t t, uint32_t u) {       // tasks t and u name the same groups >= 64 in the same order
+    if (xg_hi(t) - xg_lo(t) != xg_hi(u) - xg_lo(u)) return false;
+    for (uint32_t i = 0; i < xg_hi(t) - xg_lo(t); ++i) if (xg_at(t, i) != xg_at(u, i)) return false;
+    return true;
+  };
   if (pa) {
     aff_group_off0.assign(pa->n_groups + 1, 0);
+    uint64_t off = 0;
     for (uint32_t g = 0; g < pa->n_groups; ++g) {
       if (pa->group_keyset[g] >= pa->n_keysets) return bfail(e, KB_E_BADARG, "kb_pod_affinity: group %u names a key set out of range", g);
-      aff_group_off0[g + 1] = aff_group_off0[g] + pa->keyset_domains[pa->group_keyset[g]];
+      off += pa->keyset_domains[pa->group_keyset[g]];
+      if (off > 0xFFFFFFFFull) return bfail(e, KB_E_UNSUPPORTED_FEATURE, "kb_pod_affinity: the counters of %u groups do not fit 32-bit offsets", pa->n_groups);
+      aff_group_off0[g + 1] = (uint32_t)off;
+    }
+    if (pa->n_groups > 64 && (uint64_t)pa->n_keysets * N > 0xFFFFFFFFull)
+      return bfail(e, KB_E_UNSUPPORTED_FEATURE, "kb_pod_affinity: %u key sets x %u nodes do not fit 32-bit offsets", pa->n_keysets, N);
+    if (xg_off) {
+      for (uint32_t t = 0; t < T; ++t)
+        if (xg_off[t] > xg_off[t + 1]) return bfail(e, KB_E_BADARG, "kb_pod_affinity: task_xgroup_off is not monotone at task %u", t);
+      if (T && xg_off[T] > xg_off[0] && !pa->task_xgroup) return bfail(e, KB_E_BADARG, "kb_pod_affinity: task_xgroup is NULL but task_xgroup_off names entries");
+      for (uint32_t i = T ? xg_off[0] : 0u; T && i < xg_off[T]; ++i) {
+        const uint32_t x = pa->task_xgroup[i], g = x >> 2;
+        if (g < 64 || g >= pa->n_groups || (x & 3u) == 0)
+          return bfail(e, KB_E_BADARG, "kb_pod_affinity: task_xgroup entry %u (group %u, flags %u) is not a group >= 64 of the session", i, g, x & 3u);
+      }
     }
     const char* sw = getenv("KB_AFF_ATOMS");
     bool ok = !(sw && atoi(sw) == 0);
     const bool weights_live = hc.cf.nodeorder && hc.w_podaff != 0;
-    uint64_t used = 0;
+    uint64_t used_lo = 0;                               // groups < 64 ...
+    std::vector<uint8_t> used(pa->n_groups, 0);         // ... and every group a task reads or joins
     for (uint32_t t = 0; t < T && ok; ++t) {
       if (hc.cf.predicates && pa->task_need[t] >= 0) ok = false;
       if (weights_live && pa->task_weight_off[t + 1] > pa->task_weight_off[t]) ok = false;
-      used |= pa->task_contrib[t] | pa->task_forbid[t];
+      used_lo |= pa->task_contrib[t] | pa->task_forbid[t];
+      for (uint32_t i = xg_lo(t); i < xg_hi(t); ++i) used[xg_ent[i] >> 2] = 1;
     }
-    if (!hc.cf.predicates) used = 0;                    // step 10 is not evaluated: nothing reads the counters
-    if (pa->n_groups < 64 && (used >> pa->n_groups)) return bfail(e, KB_E_BADARG, "kb_pod_affinity: a task names a group out of range");
+    if (pa->n_groups < 64 && (used_lo >> pa->n_groups)) return bfail(e, KB_E_BADARG, "kb_pod_affinity: a task names a group out of range");
+    for (uint32_t g = 0; g < pa->n_groups && g < 64; ++g) used[g] = (uint8_t)((used_lo >> g) & 1ull);
+    if (!hc.cf.predicates) std::fill(used.begin(), used.end(), 0);    // step 10 is not evaluated: nothing reads the counters
+    uint32_t n_used = 0;
+    for (uint32_t g = 0; g < pa->n_groups; ++g) n_used += used[g];
     for (uint32_t g = 0; g < pa->n_groups && ok; ++g) {
-      if (!((used >> g) & 1ull)) continue;
+      if (!used[g]) continue;
       const uint32_t ks = pa->group_keyset[g];
       if (pa->keyset_domains[ks] != N) { ok = false; break; }
       std::vector<uint8_t> seen(N, 0);
@@ -378,14 +412,14 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
       }
     }
     int hb = -1;                                        // highest port atom in use
-    if (ok && used) {
+    if (ok && n_used) {
       for (uint32_t w = 0; w < W; ++w) {
         uint64_t acc = 0;
         for (uint32_t n = 0; n < N; ++n) acc |= s->node_ports[(size_t)w * N + n];
         for (uint32_t t = 0; t < T; ++t) acc |= s->task_port_own[(size_t)w * T + t] | s->task_port_conflict[(size_t)w * T + t];
         if (acc) hb = (int)(w * 64 + 63 - (uint32_t)__builtin_clzll(acc));
       }
-      if ((uint32_t)(hb + 1) + (uint32_t)__builtin_popcountll(used) > 64u * W) ok = false;
+      if ((uint32_t)(hb + 1) + n_used > 64u * W) ok = false;
     }
     if (ok) {
       aff_as_atoms = true;
@@ -393,7 +427,7 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
       node_aff_bits.assign((size_t)W * std::max(1u, N), 0);
       int next = hb + 1;
       for (uint32_t g = 0; g < pa->n_groups; ++g) {
-        if (!((used >> g) & 1ull)) continue;
+        if (!used[g]) continue;
         const int a = next++;
         aff_atom_of_group[g] = a;
         B.aff_atom_mask[a / 64] |= 1ull << (a % 64);
@@ -449,8 +483,11 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
       pa = &empty_pa;
     }
   }
-  auto atoms_of = [&](uint64_t groups, uint64_t* out) {
-    while (groups) { const uint32_t g = (uint32_t)__builtin_ctzll(groups); groups &= groups - 1; const int a = aff_atom_of_group[g]; if (a >= 0) out[a / 64] |= 1ull << (a % 64); }
+  // the atoms of the groups task t forbids (flag KB_XGROUP_FORBID, mask task_forbid) or joins (KB_XGROUP_CONTRIB, task_contrib)
+  auto atoms_of = [&](uint64_t groups, uint32_t t, uint32_t flag, uint64_t* out) {
+    auto put = [&](uint32_t g) { const int a = aff_atom_of_group[g]; if (a >= 0) out[a / 64] |= 1ull << (a % 64); };
+    while (groups) { const uint32_t g = (uint32_t)__builtin_ctzll(groups); groups &= groups - 1; put(g); }
+    for (uint32_t i = xg_lo(t); i < xg_hi(t); ++i) if (xg_ent[i] & flag) put(xg_ent[i] >> 2);
   };
 
   // ---------------- validate + task classes ----------------
@@ -485,16 +522,27 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
   };
   // inter-pod affinity: tasks with the same masks / kind / weight list share an "aff id", which is part of the class identity
   std::vector<uint32_t> aff_id(pa ? T : 0, 0);
-  std::vector<ClassAff> aff_tab;                  // by aff id; w_off / w_cnt index the packed lists below
+  std::vector<ClassAff> aff_tab;                  // by aff id; w_off / w_cnt, xf_off / xc_off index the packed lists below
   std::vector<int32_t> aff_wk, aff_wks; std::vector<int64_t> aff_wv;
+  std::vector<AffX> aff_xf; std::vector<uint32_t> aff_xc;
+  std::vector<uint32_t> aff_xf_group;             // host only: the group of every aff_xf entry
   if (pa) {
     std::map<std::vector<int64_t>, uint32_t> ids;
+    const bool xg_tab = pa == pa_full;            // not the empty tables of a session whose groups became atoms
     for (uint32_t t = 0; t < T; ++t) {
       std::vector<int64_t> key = {(int64_t)pa->task_forbid[t], (int64_t)pa->task_contrib[t], (int64_t)pa->task_need[t], (int64_t)pa->task_kind[t],
                                   (int64_t)((s->task_flags[t] & KB_TASK_AFF_SELF_MATCH) ? 1 : 0)};
       const uint32_t w0 = pa->task_weight_off[t], w1 = pa->task_weight_off[t + 1];
       if (w1 < w0 || w1 > pa->n_weights) return bfail(e, KB_E_BADARG, "kb_pod_affinity: task_weight_off is not monotone at task %u", t);
       for (uint32_t i = w0; i < w1; ++i) { key.push_back(pa->weight_kind[i]); key.push_back(pa->weight_keyset[i]); key.push_back(pa->weight_value[i]); }
+      // groups >= 64 belong to the identity too (after the weights, with their count in front: no key of a smaller session changes)
+      if (xg_tab && xg_hi(t) > xg_lo(t)) {
+        std::vector<int64_t> xs;
+        for (uint32_t i = xg_lo(t); i < xg_hi(t); ++i) xs.push_back(xg_ent[i]);
+        std::sort(xs.begin(), xs.end());
+        key.push_back(-(int64_t)xs.size() - 1);
+        key.insert(key.end(), xs.begin(), xs.end());
+      }
       auto it = ids.find(key);
       if (it == ids.end()) {
         if (pa->task_need[t] >= (int32_t)pa->n_groups || pa->task_kind[t] >= (int32_t)pa->n_kinds) return bfail(e, KB_E_BADARG, "kb_pod_affinity: task %u names a group / kind out of range", t);
@@ -508,6 +556,23 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
             return bfail(e, KB_E_BADARG, "kb_pod_affinity: weight entry %u names a kind / key set out of range", i);
           aff_wk.push_back(pa->weight_kind[i]); aff_wks.push_back(pa->weight_keyset[i]); aff_wv.push_back(pa->weight_value[i]);
           ca.w_keysets |= 1ull << pa->weight_keyset[i];
+        }
+        if (xg_tab && xg_hi(t) > xg_lo(t)) {
+          // forbidden groups >= 64, those the class also joins first (aff_self_blocks reads them), each resolved to (row, counters)
+          std::vector<uint32_t> both, fonly, joined;
+          for (uint32_t i = xg_lo(t); i < xg_hi(t); ++i) {
+            const uint32_t x = xg_ent[i], g = x >> 2;
+            if ((x & KB_XGROUP_FORBID) && (x & KB_XGROUP_CONTRIB)) both.push_back(g);
+            else if (x & KB_XGROUP_FORBID) fonly.push_back(g);
+            if (x & KB_XGROUP_CONTRIB) joined.push_back(g);
+          }
+          for (auto* v : {&both, &fonly, &joined}) { std::sort(v->begin(), v->end()); v->erase(std::unique(v->begin(), v->end()), v->end()); }
+          fonly.erase(std::remove_if(fonly.begin(), fonly.end(), [&](uint32_t g) { return std::binary_search(both.begin(), both.end(), g); }), fonly.end());
+          ca.xf_off = (uint32_t)aff_xf.size(); ca.xs_cnt = (uint32_t)both.size(); ca.xf_cnt = (uint32_t)(both.size() + fonly.size());
+          for (auto* v : {&both, &fonly})
+            for (const uint32_t g : *v) { aff_xf.push_back(AffX{pa->group_keyset[g] * N, aff_group_off0[g]}); aff_xf_group.push_back(g); }
+          ca.xc_off = (uint32_t)aff_xc.size(); ca.xc_cnt = (uint32_t)joined.size();
+          aff_xc.insert(aff_xc.end(), joined.begin(), joined.end());
         }
         it = ids.emplace(key, (uint32_t)aff_tab.size()).first;
         aff_tab.push_back(ca);
@@ -536,7 +601,8 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
     auto bits = [](const double* a, size_t i) { uint64_t u; memcpy(&u, a + i, 8); return u; };
     auto same_as_prev = [&](uint32_t t) {
       if (pa && aff_id[t] != aff_id[t - 1]) return false;
-      if (aff_as_atoms && (pa_full->task_forbid[t] != pa_full->task_forbid[t - 1] || pa_full->task_contrib[t] != pa_full->task_contrib[t - 1])) return false;
+      if (aff_as_atoms && (pa_full->task_forbid[t] != pa_full->task_forbid[t - 1] || pa_full->task_contrib[t] != pa_full->task_contrib[t - 1] ||
+                           !xg_same(t, t - 1))) return false;
       if (s->task_flags[t] != s->task_flags[t - 1] || s->task_n_aff_terms[t] != s->task_n_aff_terms[t - 1] ||
           s->task_nz_cpu[t] != s->task_nz_cpu[t - 1] || s->task_nz_mem[t] != s->task_nz_mem[t - 1]) return false;
       if (s->task_flags[t] & KB_TASK_HAS_PREFERRED_NODE_AFFINITY) {
@@ -592,8 +658,8 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
         for (uint32_t a = 0; a < c.n_aff; ++a) c.aff[a][w] = s->task_aff_terms[((size_t)a * W + w) * T + t];
       }
       if (aff_as_atoms) {                 // host-level anti-affinity as atoms: forbidden groups conflict, joined groups are set by Allocate
-        if (hc.cf.predicates) atoms_of(pa_full->task_forbid[t], c.port_conflict);
-        atoms_of(pa_full->task_contrib[t], c.aff_own);
+        if (hc.cf.predicates) atoms_of(pa_full->task_forbid[t], t, KB_XGROUP_FORBID, c.port_conflict);
+        atoms_of(pa_full->task_contrib[t], t, KB_XGROUP_CONTRIB, c.aff_own);
       }
       task_empty[t] = res_is_empty(R, [&](uint32_t k) { return c.resreq[k]; }) ? 1 : 0;   // allocate.go:113-118
       if (prev_class != 0xFFFFFFFFu && memcmp(&classes[prev_class], &c, sizeof c) == 0 && memcmp(&class_pref[prev_class], &cp, sizeof cp) == 0) {
@@ -635,6 +701,7 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
     if (!hc.cf.nodeorder || hc.w_podaff == 0) A.has_weights = 0;          // the priority is not registered / weighs nothing
     if (A.has_weights) hc.cf.score_bias += 10ll * (hc.w_podaff < 0 ? -(int64_t)hc.w_podaff : 0);
     A.has_pref = (B.has_pref && hc.cf.nodeorder) ? 1u : 0u;
+    A.has_x = (!aff_xf.empty() || !aff_xc.empty()) ? 1u : 0u;
     aff_keyset_off.assign(pa->n_keysets + 1, 0);
     for (uint32_t k = 0; k < pa->n_keysets; ++k) {
       if (pa->keyset_domains[k] > N) return bfail(e, KB_E_BADARG, "kb_pod_affinity: key set %u has more domains than nodes", k);
@@ -785,6 +852,8 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
     oi.aff_w_keyset = imm.alloc(std::max<size_t>(1, aff_wk.size()) * 4);
     oi.aff_w_value = imm.alloc(std::max<size_t>(1, aff_wk.size()) * 8);
     oi.aff_kind_unbound = imm.alloc(std::max(1u, pa->n_kinds));
+    oi.aff_xf = imm.alloc(std::max<size_t>(1, aff_xf.size()) * sizeof(AffX));
+    oi.aff_xc = imm.alloc(std::max<size_t>(1, aff_xc.size()) * 4);
     om.aff_cnt = mut.alloc((size_t)std::max(1u, aff_group_off[pa->n_groups]) * 4);
     om.aff_total = mut.alloc((size_t)std::max(1u, pa->n_groups) * 4);
     om.aff_kind_count = mut.alloc((size_t)std::max(1u, pa->n_kinds) * std::max(1u, N) * 4);
@@ -846,25 +915,31 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
       const uint32_t id = classes[k].flags >> 8;
       if (id < aff_tab.size()) hca[k] = aff_tab[id]; else { memset(&hca[k], 0, sizeof(ClassAff)); hca[k].need = -1; hca[k].kind = -1; }
       if (!B.aff.has_weights) { hca[k].w_cnt = 0; hca[k].w_keysets = 0; }
-      if (!hc.cf.predicates) { hca[k].forbid = 0; hca[k].need = -1; }      // step 10 belongs to the predicates plugin
+      if (!hc.cf.predicates) { hca[k].forbid = 0; hca[k].xf_cnt = 0; hca[k].xs_cnt = 0; hca[k].need = -1; }   // step 10 belongs to the predicates plugin
       // groups the class both joins and reads: if all of them live on single-node domains (and the needed group is not among
       // them: its `total` would end the first-of-series escape for every node), its own placements only change the chosen node
-      const uint64_t needbit = hca[k].need >= 0 ? (1ull << hca[k].need) : 0ull;
+      const int32_t need = hca[k].need;
+      const uint64_t needbit = (need >= 0 && need < 64) ? (1ull << need) : 0ull;
+      bool need_joined = (hca[k].contrib & needbit) != 0;
+      for (uint32_t i = 0; i < hca[k].xc_cnt && need >= 64; ++i) need_joined = need_joined || aff_xc[hca[k].xc_off + i] == (uint32_t)need;
       uint64_t m = hca[k].contrib & (hca[k].forbid | needbit);
-      bool multi = (hca[k].contrib & needbit) == 0;
+      bool multi = !need_joined;
       while (m && multi) {
         const uint32_t g = (uint32_t)__builtin_ctzll(m);
         m &= m - 1;
         multi = keyset_single[pa->group_keyset[g]] != 0;
       }
+      for (uint32_t i = 0; i < hca[k].xs_cnt && multi; ++i) multi = keyset_single[pa->group_keyset[aff_xf_group[hca[k].xf_off + i]]] != 0;
       hca[k].pred_multi_ok = multi ? 1u : 0u;
-      hca[k].self_block = (multi && (hca[k].contrib & hca[k].forbid) != 0) ? 1 : 0;
+      hca[k].self_block = (multi && ((hca[k].contrib & hca[k].forbid) != 0 || hca[k].xs_cnt != 0)) ? 1 : 0;
     }
     if (!aff_wk.empty()) {
       memcpy(ib + oi.aff_w_kind, aff_wk.data(), aff_wk.size() * 4); memcpy(ib + oi.aff_w_keyset, aff_wks.data(), aff_wks.size() * 4);
       memcpy(ib + oi.aff_w_value, aff_wv.data(), aff_wv.size() * 8);
     }
     if (pa->n_kinds) memcpy(ib + oi.aff_kind_unbound, pa->kind_unbound, pa->n_kinds);
+    if (!aff_xf.empty()) memcpy(ib + oi.aff_xf, aff_xf.data(), aff_xf.size() * sizeof(AffX));
+    if (!aff_xc.empty()) memcpy(ib + oi.aff_xc, aff_xc.data(), aff_xc.size() * 4);
     if (aff_group_off[pa->n_groups]) memcpy(mb + om.aff_cnt, pa->group_count0, (size_t)aff_group_off[pa->n_groups] * 4);
     if (pa->n_groups) memcpy(mb + om.aff_total, pa->group_total0, (size_t)pa->n_groups * 4);
     if (pa->n_kinds && N) memcpy(mb + om.aff_kind_count, pa->node_kind_count0, (size_t)pa->n_kinds * N * 4);

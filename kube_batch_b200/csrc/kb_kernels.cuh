@@ -134,9 +134,13 @@ __device__ __forceinline__ uint64_t cta_fold_lists(uint64_t mine, uint64_t (*wli
   return mine;
 }
 
+// forbidden counter groups >= 64 (ClassAff.xf_*) a scan CTA stages in shared memory: a class forbidden by more reads the rest from L2
+constexpr uint32_t AFF_XF_SMEM = 128;
+
 struct VisitSmem {
   ClassRec cls;
   ClassAff cls_aff;                          // inter-pod affinity record of the class (AFF instantiations only)
+  AffX cls_xf[AFF_XF_SMEM];                  // the first AFF_XF_SMEM entries of its forbidden-group list (AFF instantiations only)
   ClassPref cls_pref;                        // preferred node-affinity terms of the class (AFF instantiations, AffDev.has_pref)
   Ctl ctl;
   uint64_t keys[KTOP];                       // merged candidate list of the scan (K3 result)
@@ -289,7 +293,7 @@ __device__ __forceinline__ void replay_epilogue(const DevSession& S, VisitSmem& 
           if (have) {
             ColAcc acc{&sm.slot[which][0][0], (uint32_t)lane, 32u, R, W};
             eval_pair(S.cf, sm.cls, acc, my_node, nullptr, &pk);
-            if (AFF && pk && S.cf.predicates) pk = aff_pred(S.aff, sm.cls_aff, S.N, my_node);
+            if (AFF && pk && S.cf.predicates) pk = aff_pred(S.aff, sm.cls_aff, S.N, my_node);     // list entries from L2: once per task
           }
           if (S.cf.fit_mode != 2 && (sm.pred_any_all || __any_sync(FULL, pk))) {      // fit_mode 2: a node that passes the predicates is IN the list
             if (lane == 0) {
@@ -502,6 +506,10 @@ __device__ __forceinline__ uint64_t scan_phase(const DevSession& S, VisitSmem& s
       const uint32_t* as = reinterpret_cast<const uint32_t*>(&S.aff.cls[cls_id]);
       uint32_t* ad = reinterpret_cast<uint32_t*>(&sm.cls_aff);
       for (uint32_t i = tid; i < sizeof(ClassAff) / 4; i += SCAN_THREADS) ad[i] = as[i];
+      if (S.aff.has_x) {
+        const uint32_t xn = min(S.aff.cls[cls_id].xf_cnt, AFF_XF_SMEM), xo = S.aff.cls[cls_id].xf_off;
+        for (uint32_t i = tid; i < xn; i += SCAN_THREADS) sm.cls_xf[i] = S.aff.xf[xo + i];
+      }
       uint32_t* pd = reinterpret_cast<uint32_t*>(&sm.cls_pref);
       if (S.aff.has_pref) {
         const uint32_t* ps = reinterpret_cast<const uint32_t*>(&S.class_pref[cls_id]);
@@ -541,7 +549,7 @@ __device__ __forceinline__ uint64_t scan_phase(const DevSession& S, VisitSmem& s
       key = eval_pair(S.cf, sm.cls, acc, node, nullptr, PH ? &pok : nullptr);
       if (PH && pred_dead) { key = 0; pok = false; }        // a task Allocated on no node: InterPodAffinityMatches errors for every pair (Ctl.pred_dead)
       if (AFF) {
-        if (S.cf.predicates && !aff_pred(S.aff, sm.cls_aff, S.N, node)) { key = 0; pok = false; }      // predicate step 10
+        if (S.cf.predicates && !aff_pred(S.aff, sm.cls_aff, S.N, node, sm.cls_xf, AFF_XF_SMEM)) { key = 0; pok = false; }   // predicate step 10
         if (ipa && key) key = aff_add_score(key, S.aff.w_podaff, aff_score(aff_count_node(S.aff, sm.cls_aff, S.N, node), ipa_min, ipa_max));
         if (prf && key) key = add_pref_term(key, (int64_t)S.w_nodeaff, (int64_t)pref_count(sm.cls_pref, acc, S.cf.W), (int64_t)prf_max);
       }
@@ -818,6 +826,7 @@ __global__ void __launch_bounds__(AFF_THREADS)
 aff_prepass_kernel(const __grid_constant__ DevSession S) {
   __shared__ ClassRec scls;
   __shared__ ClassAff sca;
+  __shared__ AffX sxf[AFF_XF_SMEM];
   if (__ldcg(&S.ctl->done) || !S.cf.nodeorder) return;
   const uint32_t cls_id = __ldcg(&S.ctl->cur_class);
   const bool wts = S.aff.cls[cls_id].w_cnt != 0;
@@ -843,6 +852,10 @@ aff_prepass_kernel(const __grid_constant__ DevSession S) {
     const uint32_t* as = reinterpret_cast<const uint32_t*>(&S.aff.cls[cls_id]);
     uint32_t* ad = reinterpret_cast<uint32_t*>(&sca);
     for (uint32_t i = threadIdx.x; i < sizeof(ClassAff) / 4; i += blockDim.x) ad[i] = as[i];
+    if (S.aff.has_x) {
+      const uint32_t xn = min(S.aff.cls[cls_id].xf_cnt, AFF_XF_SMEM), xo = S.aff.cls[cls_id].xf_off;
+      for (uint32_t i = threadIdx.x; i < xn; i += blockDim.x) sxf[i] = S.aff.xf[xo + i];
+    }
   }
   __syncthreads();
   const size_t tile_u64 = (size_t)S.ncols * TILE_NODES;
@@ -850,7 +863,7 @@ aff_prepass_kernel(const __grid_constant__ DevSession S) {
   auto feasible = [&](const uint32_t n) {
     TileAcc acc{S.tiles + (size_t)(n / TILE_NODES) * tile_u64, n % TILE_NODES, S.cf.R, S.cf.W};
     uint64_t key = eval_pair(S.cf, scls, acc, n, nullptr);
-    if (key && S.cf.predicates && !aff_pred(S.aff, sca, S.N, n)) key = 0;
+    if (key && S.cf.predicates && !aff_pred(S.aff, sca, S.N, n, sxf, AFF_XF_SMEM)) key = 0;
     return key != 0;
   };
   if (PHASE == 1) {

@@ -270,15 +270,19 @@ def add_host_spread(s: Snapshot, frac: float = 0.1, labels: int = 8, seed: int =
     kb_pod_affinity (include/kbgpu.h) exactly as builder.flatten_pod_affinity would for such pods: per label one counter group for
     the term the pods OWN (satisfiesExistingPodsAntiAffinity) and one for the pods that MATCH the term list (the pod's own check) —
     same members, both forbidden to and joined by the label's pods; one key set (hostname: a domain per node); no pod kinds (required
-    anti-affinity terms carry no priority weight).  Pods already running carry no labels here."""
+    anti-affinity terms carry no priority weight).  Pods already running carry no labels here.  Label L owns groups 2L and 2L + 1:
+    labels 0..31 are bits of the masks, labels >= 32 entries of task_xgroup (only emitted when there are more than 64 groups)."""
     rng = np.random.Generator(np.random.PCG64(seed))
     T, N, J = s.T, s.N, s.J
     forbid = np.zeros(max(T, 1), dtype=np.uint64)
+    lab_of = np.full(max(T, 1), -1, dtype=np.int64)
     for j in range(J):
         lo, hi = int(s.job_task_off[j]), int(s.job_task_off[j + 1])
         if hi > lo and rng.random() < frac:
             lab = int(rng.integers(0, labels))
-            forbid[lo:hi] = np.uint64(3 << (2 * lab))
+            if lab < 32:
+                forbid[lo:hi] = np.uint64(3 << (2 * lab))
+            lab_of[lo:hi] = lab
             s.task_flags[lo:hi] |= abi.KB_TASK_HAS_POD_AFFINITY
     G = 2 * labels
     s.pod_affinity = {
@@ -291,7 +295,15 @@ def add_host_spread(s: Snapshot, frac: float = 0.1, labels: int = 8, seed: int =
         "task_weight_off": np.zeros(T + 1, dtype=np.uint32), "weight_kind": np.zeros(1, dtype=np.int32),
         "weight_keyset": np.zeros(1, dtype=np.int32), "weight_value": np.zeros(1, dtype=np.int64),
     }
-    s.meta["spread_tasks"] = int((forbid != 0).sum())
+    if G > 64:
+        both = abi.KB_XGROUP_FORBID | abi.KB_XGROUP_CONTRIB
+        hi_lab = lab_of[:T] >= 32
+        cnt = np.where(hi_lab, 2, 0)
+        s.pod_affinity["task_xgroup_off"] = np.concatenate([[0], np.cumsum(cnt)]).astype(np.uint32)
+        labs = lab_of[:T][hi_lab]
+        x = np.stack([((2 * labs) << 2) | both, ((2 * labs + 1) << 2) | both], axis=1).reshape(-1)
+        s.pod_affinity["task_xgroup"] = x.astype(np.uint32) if x.size else np.zeros(1, dtype=np.uint32)
+    s.meta["spread_tasks"] = int((lab_of[:T] >= 0).sum()) if T else 0
     s.invalidate()
     return s
 
