@@ -64,6 +64,7 @@ type runningFlat struct {
 	prio                               []int32
 	ctime                              []int64
 	waiting                            []int32 // [J]
+	affGroupOff, affGroup              []uint32 // [n+1] + the counter groups of each Running task
 }
 
 func (c *Cycle) flattenRunning(ssn *framework.Session, f *Flat) *runningFlat {
@@ -98,7 +99,8 @@ func (c *Cycle) flattenRunning(ssn *framework.Session, f *Flat) *runningFlat {
 	R := int(f.R)
 	r := &runningFlat{node: make([]uint32, max1(n)), job: make([]uint32, max1(n)), present: make([]uint32, max1(n)),
 		uidRank: make([]uint32, max1(n)), flags: make([]uint32, max1(n)), resreq: make([]float64, R*max1(n)),
-		prio: make([]int32, max1(n)), ctime: make([]int64, max1(n)), waiting: make([]int32, max1(len(f.JobIDs)))}
+		prio: make([]int32, max1(n)), ctime: make([]int64, max1(n)), waiting: make([]int32, max1(len(f.JobIDs))),
+		affGroupOff: make([]uint32, n+1)}
 	for i, t := range c.running {
 		r.node[i] = nodeOf[i]
 		r.job[i] = jidx[t.Job]
@@ -115,6 +117,12 @@ func (c *Cycle) flattenRunning(ssn *framework.Session, f *Flat) *runningFlat {
 				r.flags[i] |= uint32(C.KB_RUNNING_AFF_MEMBER)
 			}
 		}
+		// its counter groups (kb_running.aff_group_off / aff_group, builder.py meta["running_aff_groups"]): always filled, so the engine
+		// keeps the member bits exact when it is evicted instead of withholding the cycle
+		if f.podAff != nil && t.Pod != nil {
+			r.affGroup = append(r.affGroup, f.podAff.memberGroups[t.Pod]...)
+		}
+		r.affGroupOff[i+1] = uint32(len(r.affGroup))
 	}
 	for j, id := range f.JobIDs { // WaitingTaskNum (job_info.go:396-405): 0 unless an earlier action pipelined tasks
 		r.waiting[j] = int32(len(ssn.Jobs[id].TaskStatusIndex[api.Pipelined]))
@@ -157,6 +165,7 @@ func (c *Cycle) run(ssn *framework.Session) error {
 	run.node, run.job, run.res_present = a.u32(rf.node), a.u32(rf.job), a.u32(rf.present)
 	run.resreq, run.prio, run.ctime = a.f64(rf.resreq), a.i32(rf.prio), a.i64(rf.ctime)
 	run.uid_rank, run.flags, run.job_waiting0 = a.u32(rf.uidRank), a.u32(rf.flags), a.i32(rf.waiting)
+	run.aff_group_off, run.aff_group = a.u32(rf.affGroupOff), a.u32(append(rf.affGroup, 0)) // a.u32 needs one element
 	if rc := C.kb_session_load_running(c.engine.h, snap, run); rc != 0 {
 		if rc == C.KB_E_UNSUPPORTED_FEATURE {
 			return &ErrUnsupported{C.GoString(C.kb_last_error(c.engine.h))}

@@ -42,7 +42,8 @@ type podAff struct {
 	taskWeightOff             []uint32
 	weightKind, weightKeyset  []int32
 	weightValue               []int64
-	members                   map[*v1.Pod]bool // listed pods that are members of a counter group: KB_RUNNING_AFF_MEMBER for the Running ones
+	members                   map[*v1.Pod]bool     // listed pods that are members of a counter group: KB_RUNNING_AFF_MEMBER for the Running ones
+	memberGroups              map[*v1.Pod][]uint32 // the groups of each listed pod, ascending: kb_running.aff_group for the Running ones
 }
 
 // termProps is what a term selects: GetNamespacesFromPodAffinityTerm + LabelSelectorAsSelector (topologies.go:25-49)
@@ -401,12 +402,14 @@ func flattenPodAffinity(ssn *framework.Session, f *Flat, nidx map[string]int, sn
 	pa.groupCount0 = make([]int32, max1(gOff[len(groups)]))
 	pa.groupTotal0 = make([]int32, max1(len(groups)))
 	pa.members = map[*v1.Pod]bool{}
+	pa.memberGroups = map[*v1.Pod][]uint32{}
 	for i, p := range listed {
 		for g, gr := range groups {
 			if !gr.member[ltype[i]] {
 				continue
 			}
 			pa.members[p.pod] = true
+			pa.memberGroups[p.pod] = append(pa.memberGroups[p.pod], uint32(g))
 			pa.groupTotal0[g]++
 			if d := pa.nodeDomain[gr.keyset*N+p.node]; d >= 0 {
 				pa.groupCount0[gOff[g]+int(d)]++

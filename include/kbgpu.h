@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define KB_ABI_VERSION 2u
+#define KB_ABI_VERSION 3u
 
 /* Compile-time capacity of the dense encodings. */
 #define KB_MAX_R 8          /* resource dims: 0 = cpu (milli), 1 = memory (bytes), 2.. = scalar resources (milli) */
@@ -44,7 +44,8 @@ typedef enum kb_status {
   KB_E_STATE = -5,              /* call order violated (e.g. kb_allocate before kb_session_load) */
   KB_E_UNSUPPORTED_FEATURE = -6 /* snapshot uses a feature outside this build; kb_last_error names it (e.g. inter-pod or preferred node
                                    affinity on a sharded node axis, reclaim / preempt with inter-pod affinity beyond host-level
-                                   anti-affinity, an evicted affinity group member, an action after preempt) */
+                                   anti-affinity, an evicted affinity group member when kb_running carries no group lists, an
+                                   action after preempt) */
 } kb_status;
 
 /* node_flags bits — evaluated once by the flattener from v1.Node
@@ -232,7 +233,9 @@ typedef struct kb_snapshot {
    * Host-level anti-affinity (every group on a key set whose domains are the nodes, no required affinity, no live weights) is folded
    * into the node records and costs nothing; anything else runs on the per-visit kernels (fresh scan per task for the classes that
    * read the counters).  kb_session_load_running (reclaim / preempt) refuses sessions of the second kind (KB_E_UNSUPPORTED_FEATURE);
-   * in the first kind the evicting actions run and only the eviction of a group MEMBER (KB_RUNNING_AFF_MEMBER) withholds the outcome. ---- */
+   * in the first kind the evicting actions run.  With kb_running.aff_group_off / aff_group the engine keeps the member bits exact when a
+   * group MEMBER is evicted (and when a discarded Statement brings it back); without them such an eviction (KB_RUNNING_AFF_MEMBER)
+   * withholds the outcome. ---- */
   const kb_pod_affinity* pod_affinity;
 } kb_snapshot;
 
@@ -273,10 +276,11 @@ typedef struct kb_plugin_conf {
  */
 #define KB_RUNNING_CRITICAL (1u << 0) /* system-cluster-critical / system-node-critical priority class or kube-system namespace (conformance.go:45-53) */
 #define KB_RUNNING_AFF_MEMBER (1u << 1) /* the pod is a member of an inter-pod affinity counter group (kb_pod_affinity): evicting it takes it out of
-                                            util.PodLister and can open its topology domain for other pods.  The engine keeps host-level groups as
-                                            bits of the node records and does not clear them: when such a pod IS evicted (even inside a Statement that is
-                                            discarded later) kb_cycle / kb_reclaim / kb_preempt return KB_E_UNSUPPORTED_FEATURE instead of a result — the
-                                            shim reruns that cycle with the original actions.  Flatteners MUST set it for every Running member. */
+                                            util.PodLister and can open its topology domain for other pods.  Only read when aff_group_off is NULL:
+                                            the engine then cannot tell which member bits of the node records the eviction clears, and when such a
+                                            pod IS evicted (even inside a Statement that is discarded later) kb_cycle / kb_reclaim / kb_preempt return
+                                            KB_E_UNSUPPORTED_FEATURE instead of a result — the shim reruns that cycle with the original actions.
+                                            Flatteners MUST set it for every Running member. */
 typedef struct kb_running {
   uint32_t n;
   uint32_t reserved0;
@@ -291,6 +295,13 @@ typedef struct kb_running {
   const uint32_t* flags;        /* [n] KB_RUNNING_*                                                           */
   const int32_t*  job_waiting0; /* [J] or NULL (= 0): Pipelined tasks of the job at session open (WaitingTaskNum, job_info.go:396-405);
                                        non-zero only when an earlier action of the same cycle pipelined tasks  */
+  /* The counter groups (ids of kb_snapshot.pod_affinity) each Running task is a member of: entries aff_group_off[i] ..
+   * aff_group_off[i+1]-1 of aff_group.  With them the engine keeps the member bits of host-level groups exact through evictions
+   * and their undo, and an evicted member never withholds the outcome.  Both NULL: KB_RUNNING_AFF_MEMBER decides as before.
+   * KB_E_BADARG for non-monotone offsets, entries while aff_group is NULL, a group >= n_groups, or more listed members of a group
+   * in one topology domain than its group_count0 counter holds (that counter counts every AllocatedStatus member). */
+  const uint32_t* aff_group_off; /* [n+1] or NULL                                                            */
+  const uint32_t* aff_group;     /* [aff_group_off[n]] group ids                                             */
 } kb_running;
 
 #define KB_ENGINE_NO_OVERLAP    (1u << 0) /* never run the scan of the next visit concurrently with the replay */

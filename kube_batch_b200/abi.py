@@ -14,7 +14,7 @@ KB_ENGINE_CHAIN2 = 1 << 3
 KB_ENGINE_CHAIN4 = 1 << 4
 KB_ENGINE_NO_PIPE = 1 << 5
 KB_ENGINE_SHARD = 1 << 6
-KB_ABI_VERSION = 2
+KB_ABI_VERSION = 3
 KB_MAX_R = 8
 KB_MAX_W = 4
 KB_MAX_AFF_TERMS = 4
@@ -286,6 +286,8 @@ class kb_running(C.Structure):
         ("uid_rank", C.POINTER(C.c_uint32)),
         ("flags", C.POINTER(C.c_uint32)),
         ("job_waiting0", C.POINTER(C.c_int32)),
+        ("aff_group_off", C.POINTER(C.c_uint32)),
+        ("aff_group", C.POINTER(C.c_uint32)),
     ]
 
 
@@ -312,6 +314,16 @@ def running_to_c(running, R: int, J: int = 0):
         jw = np.ascontiguousarray(jw, dtype=np.int32)
         r.job_waiting0 = jw.ctypes.data_as(C.POINTER(C.c_int32))
         keep.append(jw)
+    # the counter groups of every Running task (builder.py meta["running_aff_groups"], merged in by the caller); NULL when absent
+    for k in ("aff_group_off", "aff_group"):
+        a = None if running is None else running.get(k)
+        if a is None:
+            continue
+        a = np.ascontiguousarray(a, dtype=np.uint32).reshape(-1)
+        if a.size == 0:
+            a = np.zeros(1, dtype=np.uint32)
+        setattr(r, k, a.ctypes.data_as(C.POINTER(C.c_uint32)))
+        keep.append(a)
     return r, keep
 
 

@@ -488,17 +488,24 @@ class SessionBuilder:
             rt["resreq"][:, i] = v
             rt["res_present"][i] = present
         pod_objects = None
+        groups_of = {}
         if any(p.pod_affinity is not None or p.pod_anti_affinity is not None for p in self.pods):
             pend_ids = set(id(p) for p in pending)
             existing = [p for p in self.pods if id(p) not in pend_ids and p.node_name in nidx and self._task_status(p) != "Pending"]
             s.pod_affinity, pod_objects = flatten_pod_affinity(nodes, pending, existing, s, on_node,
                                                                lambda p: self._task_status(p), lambda p: f"{p.namespace}/{p.group}" in jidx)
             members = s.pod_affinity.pop("member_pod_ids")
+            groups_of = s.pod_affinity.pop("member_groups")
             for i, p in enumerate(running):
                 if id(p) in members:
                     rt["flags"][i] |= abi.KB_RUNNING_AFF_MEMBER      # its eviction would take it out of util.PodLister (kbgpu.h)
-        s.meta = {"pod_objects": pod_objects, "running": rt, "nodes": [n.name for n in nodes], "tasks": [f"{p.namespace}/{p.name}" for p in pending],
-                  "jobs": list(jidx.keys()), "queues": [q.name for q in queues], "dims": dims}
+        # the counter groups of every Running task (kb_running.aff_group_off / aff_group): kept apart from "running", whose callers
+        # without them keep the withholding rule of KB_RUNNING_AFF_MEMBER; merge them in to have the member bits kept exact
+        rg = [groups_of.get(id(p), []) for p in running]
+        rag = {"aff_group_off": np.concatenate([[0], np.cumsum([len(x) for x in rg], dtype=np.int64)]).astype(np.uint32),
+               "aff_group": np.array([g for x in rg for g in x], dtype=np.uint32)}
+        s.meta = {"pod_objects": pod_objects, "running": rt, "running_aff_groups": rag, "nodes": [n.name for n in nodes],
+                  "tasks": [f"{p.namespace}/{p.name}" for p in pending], "jobs": list(jidx.keys()), "queues": [q.name for q in queues], "dims": dims}
         s.validate()
         return s
 
@@ -773,6 +780,7 @@ def flatten_pod_affinity(nodes, pending, existing, s, on_node, status_of, in_ses
     # ---- the raw objects (what a checker that walks the pods one by one needs): pending pods in task order, then the others ----
     lset, tset = set(id(p) for p in listed), set(id(p) for p in in_tasks)
     pa["member_pod_ids"] = set(id(p) for p, ty in zip(listed, ltype) if any(g_member[g][ty] for g in range(NG)))   # -> KB_RUNNING_AFF_MEMBER
+    pa["member_groups"] = {id(p): [g for g in range(NG) if g_member[g][ty]] for p, ty in zip(listed, ltype)}     # -> kb_running.aff_group
     ob = {"nodes": nodes, "pending": list(pending), "existing": list(existing), "node_index": nidx,
           "listed": [id(p) in lset for p in existing], "in_tasks": [id(p) in tset for p in existing]}
     return pa, ob

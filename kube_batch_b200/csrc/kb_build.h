@@ -237,10 +237,13 @@ struct BuiltSession {
   bool has_pref = false;             // the two-pass scan); the device slabs do not carry them yet
   AffDev aff{};                      // inter-pod (anti)affinity: sizes and flags (pointers are set by bind())
   bool aff_session = false;          // the snapshot carries kb_pod_affinity (counter path OR atoms)
-  bool aff_evict_ok = true;          // reclaim / preempt may run: no affinity tables, or host-level anti-affinity as atoms.  The bits stay
-                                     // exact as long as no MEMBER is evicted (a victim that is no member changes nothing, preemptors are
-                                     // Pipelined: never members); the eviction of a member (KB_RUNNING_AFF_MEMBER) withholds the outcome
+  bool aff_evict_ok = true;          // reclaim / preempt may run: no affinity tables, or host-level anti-affinity as atoms.  A victim that
+                                     // is no member changes nothing, preemptors are Pipelined (never members); an evicted MEMBER clears its
+                                     // atoms through the member counts of kb_evict_build.h, or withholds the outcome when kb_running carries
+                                     // no group lists (KB_RUNNING_AFF_MEMBER)
   uint64_t aff_atom_mask[KB_MAX_W] = {0};   // port-word bits that encode host-level anti-affinity groups (hidden from kb_node_state)
+  std::vector<int32_t> aff_atom_of_group;   // [n_groups] group -> port-word bit of its atom, -1 (not an atom: nobody reads or joins it);
+                                            // empty unless the session's groups became atoms
   uint32_t Tb = 0;                   // backfill order slots: Pending tasks with InitResreq.IsEmpty() (backfill.go:47)
   std::vector<uint32_t> q_alloc_present;   // [Q] scalar presence of proportion's queueAttr.allocated at session open (kb_evict.h: Resource.Less)
 
@@ -348,7 +351,8 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
   // again, every invariant of the candidate lists holds (DESIGN.md 2) and the session runs on the persistent pipeline at full
   // speed.  Not convertible (-> per-visit kernels with counters, kb_aff.h): required pod AFFINITY, live priority weights, multi-node
   // domains, nodes without the topology label, no spare bits.  KB_AFF_ATOMS=0 forces the counter path.
-  std::vector<int32_t> aff_atom_of_group;               // group -> atom index, -1
+  std::vector<int32_t>& aff_atom_of_group = B.aff_atom_of_group;   // group -> atom index, -1
+  aff_atom_of_group.clear();
   std::vector<uint64_t> node_aff_bits;                  // [W][N] initial member bits
   std::vector<uint32_t> aff_group_off0;
   bool aff_as_atoms = false;

@@ -50,7 +50,8 @@ struct EvictCtl {
   unsigned long long pairs_logical;
   // device plumbing of the master / worker kernel (kb_evict_kernels.cu): sweep mailbox, arg-max slot, the preemptor being
   // swept and its class (written by the master thread before it posts the command)
-  uint32_t cmd_seq, arrived, n_workers, pad0;
+  uint32_t cmd_seq, arrived, n_workers;
+  uint32_t fold_step;              // Allocated decisions from this step on are not yet in EvictDev.atom_cnt (evict_fold_task)
   uint32_t cls_valid, cls_id;      // class record currently in `cls`      // master -> workers: sweep command counter (~0u = exit); workers -> master: CTAs done
   uint32_t pass;                   // master -> workers: 1 = pass 1 of a preferred node-affinity class (max count), 0 = the sweep
   uint32_t pmax;                   // workers -> master (pass 1): max count; master -> workers (sweep): the normalisation max
@@ -79,6 +80,13 @@ struct EvictDev {
   const uint32_t* task_class;    // [T]
   const uint32_t* task_present;  // [T] scalar presence of the pending task's Resreq
   const int32_t*  job_waiting0;  // [J] Pipelined tasks of the job at session open (kb_running.job_waiting0)
+  // host-level anti-affinity atoms (kb_build.h) of the Running members.  r_atom_off == nullptr: kb_running carried no group lists,
+  // and evicting a KB_RUNNING_AFF_MEMBER withholds the outcome instead
+  uint32_t n_atoms;              // atoms some Running task is a member of; only these are counted
+  const uint32_t* r_atom_off;    // [n+1] slot -> its entries in r_atom
+  const uint32_t* r_atom;        // local atom indices
+  const uint32_t* atom_bit;      // [n_atoms] port-word bit of the atom
+  const int32_t*  atom_local;    // [64 * KB_MAX_W] port-word bit -> local atom index, -1 = not counted
   // mutable
   uint8_t*  r_state;             // [n] 0 Running, 1 Releasing (evicted)
   uint32_t* pt_pos;              // [J] tasks popped from preemptorTasks[job]
@@ -90,6 +98,7 @@ struct EvictDev {
   uint32_t* evict_order;         // [n] by slot: order of the cache.Evict call, 0xFFFFFFFF = not evicted
   uint32_t* ops;                 // [n + Tall] Statement.operations: bit 31 = Pipeline(task), else Evict(slot)
   uint32_t* scratch;             // [KB_EVICT_MAXV] victims of the node being committed
+  int32_t*  atom_cnt;            // [n_atoms][N] util.PodLister members per node: group_count0, + Allocated this cycle, - evicted
   EvictCtl* ctl;
 };
 
@@ -240,9 +249,19 @@ KB_HD void evict_apply(const DevSession& S, const EvictDev& E, const uint32_t no
   const size_t tile_u64 = (size_t)S.ncols * TILE_NODES;
   uint64_t* t = S.tiles + (size_t)(node / TILE_NODES) * tile_u64 + (node % TILE_NODES);
   E.r_state[slot] = undo ? 0 : 1;
-  // KB_RUNNING_AFF_MEMBER: the victim leaves util.PodLister — the member bits of the node records (host-level inter-pod
-  // anti-affinity as atoms, kb_build.h) would have to change with it.  They do not: the cycle's outcome is withheld (error 3).
-  if (!undo && (E.r_flags[slot] & KB_RUNNING_AFF_MEMBER) && E.ctl->error == 0) E.ctl->error = 3;
+  // A member leaves util.PodLister when evicted (and comes back with a discarded Statement): the member bits of the node record
+  // (host-level inter-pod anti-affinity as atoms, kb_build.h) follow its counts.  The workers read the record only after the
+  // next command word, so the sweep that follows sees the change.  Without group lists the outcome is withheld (error 3).
+  if (E.r_atom_off) {
+    for (uint32_t i = E.r_atom_off[slot]; i < E.r_atom_off[slot + 1]; ++i) {
+      const uint32_t l = E.r_atom[i], a = E.atom_bit[l];
+      int32_t& cnt = E.atom_cnt[(size_t)l * S.N + node];
+      cnt += undo ? 1 : -1;
+      uint64_t& pw = t[(size_t)col_ports(R, S.cf.W, a / 64) * TILE_NODES];
+      if (cnt == 0) pw &= ~(1ull << (a % 64));
+      else if (undo && cnt == 1) pw |= 1ull << (a % 64);
+    }
+  } else if (!undo && (E.r_flags[slot] & KB_RUNNING_AFF_MEMBER) && E.ctl->error == 0) E.ctl->error = 3;
   S.job_ready[j] += undo ? 1 : -1;                                         // Running counts as ready, Releasing does not (job_info.go:383-393)
   for (uint32_t k = 0; k < R; ++k) {
     const double r = E.r_resreq[(size_t)k * n + slot];
@@ -430,12 +449,33 @@ struct CpuExec {
 // Start of an evicting action (reclaim.go:47-81, preempt.go:47-75): the action's own queues are filled from the session as it
 // is NOW — jobs in the canonical job order, Go container/heap pushes with the comparators on the current state; a job
 // enters with the tasks it still has in TaskStatusIndex[Pending].  Thread 0 only (J pushes of O(log J)).
-// WaitingTaskNum and the cursor on the first Pending task of job j, from the decision table as the earlier actions left it
+// WaitingTaskNum and the cursor on the first Pending task of job j, from the decision table as the earlier actions left it;
+// the same walk folds the job's Allocated members into the atom counts
+// A task an earlier allocate / backfill of this cycle Allocated on a node is a member of the groups its class joins (the
+// ClassRec.aff_own bits those placements OR into the record): its atoms' counts on that node go up by one before any eviction
+// reads them.  Only decisions from ctl.fold_step on count: an earlier evicting action of the cycle folded the ones before.
+KB_HD void evict_fold_task(const DevSession& S, const EvictDev& E, const uint32_t t) {
+  const kb_decision d = S.dec[t];
+  if (d.kind != KB_KIND_ALLOCATED || d.node < 0 || d.step < E.ctl->fold_step) return;     // phantom backfill tasks: no node
+  const ClassRec& c = S.classes[E.task_class[t]];
+  for (uint32_t w = 0; w < S.cf.W; ++w)
+    for (uint64_t m = c.aff_own[w]; m; m &= m - 1) {
+#if defined(__CUDA_ARCH__)
+      const int32_t l = E.atom_local[w * 64 + (uint32_t)(__ffsll((long long)m) - 1)];
+      if (l >= 0) atomicAdd(&E.atom_cnt[(size_t)l * S.N + (uint32_t)d.node], 1);
+#else
+      const int32_t l = E.atom_local[w * 64 + (uint32_t)__builtin_ctzll(m)];
+      if (l >= 0) E.atom_cnt[(size_t)l * S.N + (uint32_t)d.node] += 1;
+#endif
+    }
+}
+
 KB_HD void evict_scan_job(const DevSession& S, const EvictDev& E, const uint32_t j) {
   int32_t w = E.job_waiting0[j];
   uint32_t first = 0xFFFFFFFFu;
   for (uint32_t i = E.pt_off[j]; i < E.pt_off[j + 1]; ++i) {
     const uint32_t t = E.pt_task[i];
+    if (E.n_atoms) evict_fold_task(S, E, t);
     if (S.dec[t].kind == KB_KIND_PIPELINED) w += 1;                  // WaitingTaskNum (job_info.go:396-405)
     if (first == 0xFFFFFFFFu && task_pending(S, t)) first = i - E.pt_off[j];
   }
@@ -455,6 +495,7 @@ KB_HD void evict_init(X& x, const DevSession& S, const EvictDev& E) {
     auto qless = [&](uint32_t l, uint32_t r) { return queue_before(S, l, r); };
     auto jless = [&](uint32_t l, uint32_t r) { return job_before(S, l, r); };
     ctl.qheap_len = 0; ctl.n_ops = 0; ctl.fail_valid = 0;
+    ctl.fold_step = ctl.step;                                   // every Allocate of the cycle so far is in atom_cnt now
     for (uint32_t q = 0; q < S.Q; ++q) { E.jheap_len[q] = 0; E.scratch[q] = 0; }    // scratch doubles as queueMap (Q <= KB_MAX_Q <= KB_EVICT_MAXV)
     for (uint32_t j = 0; j < S.J; ++j) {
       const uint32_t q = S.job_queue[j];

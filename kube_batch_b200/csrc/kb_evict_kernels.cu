@@ -171,7 +171,7 @@ evict_kernel(const __grid_constant__ DevSession S, const __grid_constant__ Evict
   }
 }
 
-// evict_init's per-job scan (WaitingTaskNum, first Pending task), one thread per job
+// evict_init's per-job scan (WaitingTaskNum, first Pending task, the job's Allocated members into the atom counts), one thread per job
 __global__ void evict_scan_kernel(const __grid_constant__ DevSession S, const __grid_constant__ EvictDev E) {
   const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
   if (j < S.J) evict_scan_job(S, E, j);

@@ -308,6 +308,31 @@ def add_host_spread(s: Snapshot, frac: float = 0.1, labels: int = 8, seed: int =
     return s
 
 
+def add_running_members(s: Snapshot, run: dict, frac: float = 0.1, labels: int = 8, seed: int = 13) -> dict:
+    """After add_host_spread: makes `frac` of the Running tasks `run` (running_of) replicas of the spread Deployments — each carries
+    app=<L> and the label's required anti-affinity term, so it is a member of both groups of label L (2L, 2L + 1).  Updates
+    group_count0 / group_total0 of the snapshot and KB_RUNNING_AFF_MEMBER of `run` in place, and returns the per-task group lists
+    (kb_running.aff_group_off / aff_group) in the format builder.flatten emits under meta["running_aff_groups"]."""
+    rng = np.random.Generator(np.random.PCG64(seed))
+    pa, N = s.pod_affinity, s.N
+    n = len(run["node"])
+    lab = np.where(rng.random(n) < frac, rng.integers(0, labels, size=n), -1)
+    off = np.zeros(n + 1, dtype=np.uint32)
+    groups = []
+    for i in range(n):
+        if lab[i] >= 0:
+            g = [2 * int(lab[i]), 2 * int(lab[i]) + 1]
+            groups += g
+            for x in g:
+                pa["group_count0"][x * N + int(run["node"][i])] += 1
+                pa["group_total0"][x] += 1
+            run["flags"][i] |= abi.KB_RUNNING_AFF_MEMBER
+        off[i + 1] = len(groups)
+    s.meta["member_tasks"] = int((lab >= 0).sum())
+    s.invalidate()
+    return {"aff_group_off": off, "aff_group": np.array(groups, dtype=np.uint32)}
+
+
 def add_node_pref(s: Snapshot, frac: float = 0.3, seed: int = 11) -> Snapshot:
     """Gives `frac` of the PodGroups the preferred zone affinity Helm charts and operators commonly set: every pod of the group carries
     1-3 nodeAffinity.preferredDuringSchedulingIgnoredDuringExecution terms {zone In [z]} with weights from {1, 10, 50, 100}.  The zones
