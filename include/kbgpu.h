@@ -232,8 +232,12 @@ typedef struct kb_snapshot {
   /* ---- inter-pod (anti)affinity (predicate step 10 + InterPodAffinityPriority), NULL = no pod of the session carries terms.
    * Host-level anti-affinity (every group on a key set whose domains are the nodes, no required affinity, no live weights) is folded
    * into the node records and costs nothing; anything else runs on the per-visit kernels (fresh scan per task for the classes that
-   * read the counters).  kb_session_load_running (reclaim / preempt) refuses sessions of the second kind (KB_E_UNSUPPORTED_FEATURE);
-   * in the first kind the evicting actions run.  With kb_running.aff_group_off / aff_group the engine keeps the member bits exact when a
+   * read the counters).  kb_session_load_running (reclaim / preempt) refuses sessions of the second kind (KB_E_UNSUPPORTED_FEATURE)
+   * when a pending task's class reads a counter group in predicate step 10 (the predicates plugin is on and the task has task_forbid
+   * bits, KB_XGROUP_FORBID entries or task_need >= 0): the victim walk does not follow an evicted member out of the groups.  Sessions
+   * of the second kind whose groups nobody reads (soft (anti)affinity: only InterPodAffinityPriority reads the tables) run the evicting
+   * actions, with the priority in preempt's node order and the Pipelined preemptors counted; evicting a member of an unread group is
+   * not observable there and never withholds the outcome.  In the first kind the evicting actions run.  With kb_running.aff_group_off / aff_group the engine keeps the member bits exact when a
    * group MEMBER is evicted (and when a discarded Statement brings it back); without them such an eviction (KB_RUNNING_AFF_MEMBER)
    * withholds the outcome. ---- */
   const kb_pod_affinity* pod_affinity;

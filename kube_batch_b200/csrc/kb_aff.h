@@ -242,6 +242,11 @@ KB_HD void aff_commit(const AffDev& A, const ClassAff& ca, const uint32_t N, con
   const int32_t fu = KB_LDM(A.first_unbound);
   if (fu < 0 || (int32_t)n < fu) *A.first_unbound = (int32_t)n;
 }
+// Statement.unpipeline of such a task (node.RemoveTask): its kind count on n goes down again.  first_unbound is a min over the
+// placed pods and cannot be undone here: the caller restores the value it saved when the Statement opened.
+KB_HD void aff_unpipeline(const AffDev& A, const ClassAff& ca, const uint32_t N, const uint32_t n) {
+  if (ca.kind >= 0) A.kind_count[(size_t)ca.kind * N + n] = KB_LDM(&A.kind_count[(size_t)ca.kind * N + n]) - 1;
+}
 
 }  // namespace kb
 #endif  // KB_AFF_H_

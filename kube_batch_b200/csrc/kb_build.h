@@ -240,7 +240,11 @@ struct BuiltSession {
   bool aff_evict_ok = true;          // reclaim / preempt may run: no affinity tables, or host-level anti-affinity as atoms.  A victim that
                                      // is no member changes nothing, preemptors are Pipelined (never members); an evicted MEMBER clears its
                                      // atoms through the member counts of kb_evict_build.h, or withholds the outcome when kb_running carries
-                                     // no group lists (KB_RUNNING_AFF_MEMBER)
+                                     // no group lists (KB_RUNNING_AFF_MEMBER).  On the counter path: no class reads a counter group in
+                                     // predicate step 10 (aff_groups_unread); the evicting actions then keep kind_count / first_unbound
+                                     // of InterPodAffinityPriority (kb_evict.h)
+  bool aff_groups_unread = false;    // counter path, and no class has forbid / xf_cnt / need >= 0 with the predicates plugin on: a
+                                     // member's eviction (it leaves util.PodLister) changes nothing any predicate reads
   uint64_t aff_atom_mask[KB_MAX_W] = {0};   // port-word bits that encode host-level anti-affinity groups (hidden from kb_node_state)
   std::vector<int32_t> aff_atom_of_group;   // [n_groups] group -> port-word bit of its atom, -1 (not an atom: nobody reads or joins it);
                                             // empty unless the session's groups became atoms
@@ -342,6 +346,7 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
   if (rc) return rc;
   B.aff_session = pa != nullptr;
   B.aff_evict_ok = pa == nullptr;
+  B.aff_groups_unread = false;
   for (uint32_t w = 0; w < KB_MAX_W; ++w) B.aff_atom_mask[w] = 0;
   // Host-level inter-pod anti-affinity as ATOMS.  When every counter the session's tasks read or join lives on a key set whose
   // domains are exactly the nodes (kubernetes.io/hostname), "a member of group g sits in the node's domain" is a per-node bit,
@@ -584,6 +589,16 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
       aff_id[t] = it->second;
     }
     if (aff_tab.size() >= (1u << 24)) return bfail(e, KB_E_UNSUPPORTED_FEATURE, "kb_pod_affinity: too many distinct affinity signatures");
+    // Counter path: reclaim / preempt run when no class reads a counter group in predicate step 10.  The victim walk does not
+    // follow the groups (an evicted member leaves util.PodLister), but then nothing reads them; InterPodAffinityPriority reads
+    // NodeInfo.Tasks, which keeps an evicted pod as Releasing, and the evicting actions keep its kind counts (kb_evict.h).
+    if (pa == pa_full && !aff_as_atoms) {
+      bool reads = false;
+      if (hc.cf.predicates)
+        for (const ClassAff& ca : aff_tab) reads = reads || ca.forbid != 0 || ca.xf_cnt != 0 || ca.need >= 0;
+      B.aff_groups_unread = !reads;
+      B.aff_evict_ok = !reads;
+    }
   }
   std::vector<uint32_t> task_class(T, 0);
   std::vector<uint8_t> task_empty(T, 0);

@@ -682,6 +682,7 @@ int kb_session_load_running(kb_engine* e, const kb_snapshot* s, const kb_running
   if (!s || s->N != e->N || s->T != e->T || s->J != e->J || s->Q != e->Q || s->R != e->R)
     return fail(e, KB_E_BADARG, "kb_session_load_running: `snap` is not the snapshot of the loaded session");
   if (e->world > 1 && !e->replicated) return fail(e, KB_E_UNSUPPORTED_FEATURE, "reclaim / preempt run on the full node table: not with KB_ENGINE_SHARD");
+  // counter path: refused when a pending class reads a counter group in predicate step 10 (kb_build.h aff_groups_unread)
   if (e->built.aff_session && !e->built.aff_evict_ok)
     return fail(e, KB_E_UNSUPPORTED_FEATURE, "reclaim / preempt in this session with inter-pod affinity are outside this build: the victim walk does not "
                 "update the affinity counters (only host-level anti-affinity, kept as bits of the node records, runs the evicting actions)");

@@ -6,7 +6,8 @@
 //
 // Shape of the work: per PREEMPTOR task one pass over all nodes — ssn.PredicateFn (K1, the same eval_pair as allocate),
 // for preempt also the node score (K2, util.PrioritizeNodes + util.SortNodes == arg-max of the packed key; a class with preferred
-// node-affinity terms first takes one more pass over all nodes for NodeAffinityPriority's max count), and per node a
+// node-affinity terms first takes one more pass over all nodes for NodeAffinityPriority's max count, a class with an inter-pod
+// weight list two more for InterPodAffinityPriority's weights per domain and min / max count), and per node a
 // short SERIAL walk over the node's Running tasks (the plugins' filters are order-dependent: drf / proportion subtract
 // cumulatively) -> "first node in order whose victims cover InitResreq".  The node axis is data-parallel (one thread per
 // node, block arg-max); the commit on the chosen node (evictions, Pipeline, Statement log) is serial.  The control flow
@@ -53,9 +54,13 @@ struct EvictCtl {
   uint32_t cmd_seq, arrived, n_workers;
   uint32_t fold_step;              // Allocated decisions from this step on are not yet in EvictDev.atom_cnt (evict_fold_task)
   uint32_t cls_valid, cls_id;      // class record currently in `cls`      // master -> workers: sweep command counter (~0u = exit); workers -> master: CTAs done
-  uint32_t pass;                   // master -> workers: 1 = pass 1 of a preferred node-affinity class (max count), 0 = the sweep
+  uint32_t pass;                   // master -> workers: 1 = pass 1 of a preferred node-affinity class (max count), 0 = the sweep;
+                                   //   2 / 3 / 4 = InterPodAffinityPriority: clear dom_sum, weights per domain, min / max count (+ pmax)
   uint32_t pmax;                   // workers -> master (pass 1): max count; master -> workers (sweep): the normalisation max
+  int32_t  stmt_fu;                // AffDev.first_unbound when the open Statement started (restored by its Discard)
+  uint32_t pad0;
   unsigned long long red;
+  long long amin, amax;            // workers -> master (pass 4): min / max InterPodAffinityPriority count; master -> workers (sweep)
   Preemptor pre;
   ClassRec cls;
 };
@@ -195,24 +200,51 @@ KB_HD const ClassPref* evict_pref(const DevSession& S, const Preemptor& P) {
   return (P.mode != 0 && S.class_pref != nullptr && S.cf.nodeorder && S.class_pref[P.cls].n != 0) ? &S.class_pref[P.cls] : nullptr;
 }
 
+// The weight list InterPodAffinityPriority reads for this preemptor (registered by nodeorder with podaffinity.weight != 0: the
+// host build zeroes every list otherwise), nullptr when the score has no such term.  Only sessions whose classes read no counter
+// group get here with a list (BuiltSession.aff_groups_unread), so ssn.PredicateFn needs no step 10 below.
+KB_HD const ClassAff* evict_aff(const DevSession& S, const Preemptor& P) {
+  return (P.mode != 0 && S.aff.on && S.aff.has_weights && S.cf.nodeorder && S.aff.cls[P.cls].w_cnt != 0) ? &S.aff.cls[P.cls] : nullptr;
+}
+
+// ssn.PredicateFn (K1 without the Idle test: preempt never checks Idle) on one node
+KB_HD bool evict_pred_ok(const DevSession& S, const ClassRec& c, const uint32_t node) {
+  const size_t tile_u64 = (size_t)S.ncols * TILE_NODES;
+  TileAcc acc{S.tiles + (size_t)(node / TILE_NODES) * tile_u64, node % TILE_NODES, S.cf.R, S.cf.W};
+  bool pok = true;
+  (void)eval_pair(S.cf, c, acc, node, nullptr, &pok);
+  return pok;
+}
+
 // Pass 1 for such a preemptor, per node: its NodeAffinityPriority count when the node passes ssn.PredicateFn, else 0.
 // NormalizeReduce divides by the max count over util.PredicateNodes (preempt.go:180-189, reduce.go:28-63), i.e. over EVERY node
 // that passes the predicates — also nodes without Running tasks or eligible victims, and full nodes (preempt never checks Idle) —
 // so this runs on all nodes, not only on those evict_node_key gives a key.  The max starts at 0, so 0 stands for "not counted".
 KB_HD uint32_t evict_pref_count(const DevSession& S, const ClassRec& c, const ClassPref& cp, const uint32_t node) {
+  if (!evict_pred_ok(S, c, node)) return 0;
   const size_t tile_u64 = (size_t)S.ncols * TILE_NODES;
   TileAcc acc{S.tiles + (size_t)(node / TILE_NODES) * tile_u64, node % TILE_NODES, S.cf.R, S.cf.W};
-  bool pok = true;
-  (void)eval_pair(S.cf, c, acc, node, nullptr, &pok);
-  if (!pok) return 0;
   const int32_t cnt = pref_count(cp, acc, S.cf.W);
   return cnt > 0 ? (uint32_t)cnt : 0u;
 }
 
+// What the node order of one preempt sweep adds to the resource scores, from the passes before it:
+//   cp / pmax     NodeAffinityPriority: evict_pref and the max of evict_pref_count over all nodes
+//   ca / amin / amax  InterPodAffinityPriority (interpod_affinity.go:99-235): evict_aff; AffDev.dom_sum holds the weights per
+//                 domain of the pods on every node that passes ssn.PredicateFn (aff_pass1_node), amin / amax the min / max of
+//                 aff_count_node over the same nodes (both start at 0).  The pods are NodeInfo.Tasks: an evicted pod stays there
+//                 as Releasing (no count changes), a Pipelined one is added (pipeline_apply).
+struct EvictPrio {
+  const ClassPref* cp;
+  uint32_t pmax;
+  const ClassAff* ca;
+  long long amin, amax;
+};
+
 // K1 (+K2 for preempt) + the victim walk of one node: packed key (score, node) if the node's victims cover InitResreq, else 0.
-// cp / pmax: evict_pref and the max of evict_pref_count over all nodes (pass 1); the score gains 10 * count / pmax times
-// nodeaffinity.weight (a negative weight is already folded into cf.score_bias).
-KB_HD uint64_t evict_node_key(const DevSession& S, const EvictDev& E, const Preemptor& P, const ClassRec& c, const ClassPref* cp, const uint32_t pmax,
+// The score gains nodeaffinity.weight * (10 * count / pmax) and podaffinity.weight * aff_score (negative weights are already
+// folded into cf.score_bias).
+KB_HD uint64_t evict_node_key(const DevSession& S, const EvictDev& E, const Preemptor& P, const ClassRec& c, const EvictPrio& pr,
                               const uint32_t node, uint32_t* err) {
   const uint32_t R = S.cf.R, W = S.cf.W, n = E.n_run;
   const uint32_t lo = E.node_off[node], hi = E.node_off[node + 1];
@@ -237,8 +269,10 @@ KB_HD uint64_t evict_node_key(const DevSession& S, const EvictDev& E, const Pree
   if (nv == 0) return 0;                                                   // reclaim.go:141-144 / validateVictims
   if (!res_less_equal(R, [&](uint32_t k) { return c.initreq[k]; }, [&](uint32_t k) { return all[k]; })) return 0;   // :147-154
   if (P.mode == 0) return pack_key(S.cf.score_bias, node);
-  const uint64_t key = pack_key(node_score(S.cf, c, acc), node);          // util.SortNodes: best score first, node order among equals
-  return cp ? add_pref_term(key, (int64_t)S.w_nodeaff, (int64_t)pref_count(*cp, acc, W), (int64_t)pmax) : key;
+  uint64_t key = pack_key(node_score(S.cf, c, acc), node);                // util.SortNodes: best score first, node order among equals
+  if (pr.cp) key = add_pref_term(key, (int64_t)S.w_nodeaff, (int64_t)pref_count(*pr.cp, acc, W), (int64_t)pr.pmax);
+  if (pr.ca) key = aff_add_score(key, S.aff.w_podaff, aff_score(aff_count_node(S.aff, *pr.ca, S.N, node), pr.amin, pr.amax));
+  return key;
 }
 
 // ---- state changes (thread 0) ----
@@ -310,6 +344,13 @@ KB_HD void pipeline_apply(const DevSession& S, const EvictDev& E, const Preempto
   }
   if (S.drf_present) update_job_share(S, j);
   if (S.proportion_present) update_queue_share(S, q);
+  // counter path: node.AddTask puts the pod into NodeInfo.Tasks, which InterPodAffinityPriority reads for every later pod of the
+  // cycle (its Spec.NodeName stays "": cachedNodeInfo.GetNodeInfo's first_unbound).  Pipelined is no AllocatedStatus: no group
+  // counter moves.  The undo's first_unbound is restored by the caller (EvictCtl.stmt_fu).
+  if (S.aff.on) {
+    if (!undo) aff_commit(S.aff, S.aff.cls[P.cls], S.N, node, false);
+    else aff_unpipeline(S.aff, S.aff.cls[P.cls], S.N, node);
+  }
   kb_decision d;
   d.node = undo ? -1 : (int32_t)node;
   d.kind = undo ? (res_is_empty(R, [&](uint32_t k) { return c.resreq[k]; }) ? KB_KIND_SKIPPED : KB_KIND_NONE) : KB_KIND_PIPELINED;
@@ -432,13 +473,22 @@ struct CpuExec {
   KB_HD bool jobs_scanned() const { return false; }
   KB_HD void clear_max() {}
   uint64_t sweep(const DevSession& S, const EvictDev& E, const Preemptor& P, const ClassRec& c) {      // the node axis, serially
-    const ClassPref* cp = evict_pref(S, P);
-    uint32_t pmax = 0;
-    if (cp)                                                       // pass 1 (preferred terms only): the normalisation max, on the current records
-      for (uint32_t n = 0; n < S.N; ++n) { const uint32_t v = evict_pref_count(S, c, *cp, n); pmax = v > pmax ? v : pmax; }
+    EvictPrio pr{evict_pref(S, P), 0u, evict_aff(S, P), 0ll, 0ll};
+    if (pr.ca) {                                                  // InterPodAffinityPriority: weights per domain, then min / max (+ pmax)
+      for (uint32_t i = 0; i < S.aff.dom_total; ++i) S.aff.dom_sum[i] = 0;
+      for (uint32_t n = 0; n < S.N; ++n)
+        if (evict_pred_ok(S, c, n)) aff_pass1_node(S.aff, *pr.ca, S.N, n, [&](uint32_t slot, long long v) { S.aff.dom_sum[slot] += v; });
+      for (uint32_t n = 0; n < S.N; ++n) {
+        if (!evict_pred_ok(S, c, n)) continue;
+        const long long cnt = aff_count_node(S.aff, *pr.ca, S.N, n);
+        pr.amin = cnt < pr.amin ? cnt : pr.amin; pr.amax = cnt > pr.amax ? cnt : pr.amax;
+        if (pr.cp) { const uint32_t v = evict_pref_count(S, c, *pr.cp, n); pr.pmax = v > pr.pmax ? v : pr.pmax; }
+      }
+    } else if (pr.cp)                                             // pass 1 (preferred terms only): the normalisation max, on the current records
+      for (uint32_t n = 0; n < S.N; ++n) { const uint32_t v = evict_pref_count(S, c, *pr.cp, n); pr.pmax = v > pr.pmax ? v : pr.pmax; }
     uint64_t best = 0;
     uint32_t err = 0;
-    for (uint32_t n = 0; n < S.N; ++n) { const uint64_t k = evict_node_key(S, E, P, c, cp, pmax, n, &err); best = k > best ? k : best; }
+    for (uint32_t n = 0; n < S.N; ++n) { const uint64_t k = evict_node_key(S, E, P, c, pr, n, &err); best = k > best ? k : best; }
     if (err) E.ctl->error = err;
     return best;
   }
@@ -545,7 +595,8 @@ KB_HD bool try_preemptor(X& x, const DevSession& S, const EvictDev& E, const uin
   const Preemptor& P = x.pre();
   const ClassRec& c = x.cls();
   // An identical sweep (same class, same filter, nothing changed since) that found no node finds none again: skip it.  This holds
-  // with preferred node-affinity terms too: their scores only order the valid nodes, whether a valid node exists does not depend on them.
+  // with preferred node-affinity terms and inter-pod weights too: their scores only order the valid nodes, whether a valid node exists
+  // does not depend on them (and a Pipeline, which moves the kind counts, bumps ctl.version).
   const uint32_t fkey = mode == 0 ? P.queue : job;
   const bool known_fail = ctl.fail_valid && ctl.fail_cls == P.cls && ctl.fail_mode == mode && ctl.fail_key == fkey && ctl.fail_version == ctl.version;
   uint64_t best = 0;
@@ -606,6 +657,7 @@ KB_HD void run_preempt(X& x, const DevSession& S, const EvictDev& E) {
     for (;;) {
       uint32_t pj = 0xFFFFFFFFu;
       if (x.tid() == 0 && E.jheap_len[q] != 0) pj = heap_pop(jh, E.jheap_len[q], jless);      // :83-88
+      if (x.tid() == 0 && S.aff.on) ctl.stmt_fu = KB_LDM(S.aff.first_unbound);                 // :90 ssn.Statement()
       pj = x.bcast(pj);
       if (pj == 0xFFFFFFFFu || ctl.error) break;
       bool assigned = false;
@@ -639,6 +691,7 @@ KB_HD void run_preempt(X& x, const DevSession& S, const EvictDev& E) {
               evict_apply(S, E, lo, op, true);
             }
           }
+          if (S.aff.on) *S.aff.first_unbound = ctl.stmt_fu;     // the Statement's evictions never move it, its Pipelines only lower it
           ctl.n_ops = 0;
         } else if (assigned) heap_push(jh, E.jheap_len[q], pj, jless);     // :133-135
       }

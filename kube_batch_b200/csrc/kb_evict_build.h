@@ -17,6 +17,7 @@ struct EvictBuilt {
   struct { size_t r_state, pt_pos, job_waiting, jheap, jheap_len, qheap, q_alloc_present, evict_order, ops, scratch, ctl, atom_cnt; } om;
   uint32_t n_run = 0, Tall = 0;
   bool lists = false;                // kb_running carried aff_group_off: the atoms of the members are counted
+  bool groups_unread = false;        // BuiltSession.aff_groups_unread: a member's eviction changes nothing observable (empty atom lists)
   uint32_t n_atoms = 0;
   EvictConf ec{};
   void bind(EvictDev& E, unsigned char* ib, unsigned char* mb) const {
@@ -28,7 +29,7 @@ struct EvictBuilt {
     E.task_class = (const uint32_t*)(ib + oi.task_class); E.task_present = (const uint32_t*)(ib + oi.task_present);
     E.job_waiting0 = (const int32_t*)(ib + oi.job_waiting0);
     E.n_atoms = n_atoms;
-    E.r_atom_off = lists ? (const uint32_t*)(ib + oi.r_atom_off) : nullptr; E.r_atom = (const uint32_t*)(ib + oi.r_atom);
+    E.r_atom_off = (lists || groups_unread) ? (const uint32_t*)(ib + oi.r_atom_off) : nullptr; E.r_atom = (const uint32_t*)(ib + oi.r_atom);
     E.atom_bit = (const uint32_t*)(ib + oi.atom_bit); E.atom_local = (const int32_t*)(ib + oi.atom_local);
     E.atom_cnt = (int32_t*)(mb + om.atom_cnt);
     E.r_state = (uint8_t*)(mb + om.r_state); E.pt_pos = (uint32_t*)(mb + om.pt_pos); E.job_waiting = (int32_t*)(mb + om.job_waiting);
@@ -77,6 +78,7 @@ inline int build_evict(const kb_snapshot* s, const kb_running* run, const BuiltS
   }
   EB.n_run = n;
   EB.lists = lists;
+  EB.groups_unread = B.aff_groups_unread;      // r_atom_off stays all zero without lists: no member has an atom
   EB.ec.reclaim_fns = B.hc.reclaim_fns; EB.ec.preempt_fns = B.hc.preempt_fns;
   EB.ec.gang_pipelined = B.hc.gang_pipelined ? 1u : 0u; EB.ec.task_order_priority = B.hc.task_order_priority ? 1u : 0u;
   // ---- Running tasks: CSR by node, UID order inside a node ----

@@ -13,6 +13,11 @@
 //           before its sweep: the workers reduce the NodeAffinityPriority max count over all their nodes (warp REDUX.MAX, one
 //           atomicMax per CTA into EvictCtl.pmax) and arrive; the sweep command that follows reads pmax from the mailbox.  Workers
 //           keep the class's ClassPref in shared memory and copy it only when the class changes.
+//   passes 2-4  a preempting class with an inter-pod weight list (evict_aff, InterPodAffinityPriority) takes three round trips
+//           instead: 2 clears AffDev.dom_sum, 3 adds the weights of the pods on every node that passes ssn.PredicateFn to their
+//           domains (64-bit integer atomicAdd: the sums do not depend on the order), 4 reduces the min / max count over the same
+//           nodes (warp REDUX on both halves, one atomicMin / atomicMax per CTA into EvictCtl.amin / amax) and, for a class that
+//           also has preferred node-affinity terms, pmax in the same pass.  Classes without a list post exactly what they did before.
 //
 // Coherence: the master mutates node records, job / queue accounting and the Running tasks' states between two sweeps.  It
 // publishes them with a release store of the command word; thread 0 of every worker CTA reads that word with ld.acquire.gpu —
@@ -34,6 +39,23 @@ __device__ __forceinline__ uint32_t ev_ld_acquire(const uint32_t* p) {
 }
 __device__ __forceinline__ void ev_st_release(uint32_t* p, uint32_t v) {
   asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+
+// min / max of a signed 64-bit value over the warp with two 32-bit REDUX each: the high words (signed), then the low words
+// (unsigned) of the lanes that hold the winning high word
+__device__ __forceinline__ long long ev_warp_max(const long long v) {
+  const int hi = (int)(v >> 32);
+  const unsigned lo = (unsigned)v;
+  const int mhi = __reduce_max_sync(0xFFFFFFFFu, hi);
+  const unsigned mlo = __reduce_max_sync(0xFFFFFFFFu, hi == mhi ? lo : 0u);
+  return (long long)(((unsigned long long)(unsigned)mhi << 32) | mlo);
+}
+__device__ __forceinline__ long long ev_warp_min(const long long v) {
+  const int hi = (int)(v >> 32);
+  const unsigned lo = (unsigned)v;
+  const int mhi = __reduce_min_sync(0xFFFFFFFFu, hi);
+  const unsigned mlo = __reduce_min_sync(0xFFFFFFFFu, hi == mhi ? lo : 0xFFFFFFFFu);
+  return (long long)(((unsigned long long)(unsigned)mhi << 32) | mlo);
 }
 
 // the master thread's Exec: single-threaded control, the sweep is farmed out
@@ -60,7 +82,9 @@ struct MasterExec {
   __device__ __forceinline__ uint64_t sweep(const DevSession& S, const EvictDev&, const Preemptor& P, const ClassRec&) {
     // preferred node-affinity terms: pass 1 leaves the max count in g->pmax, which is then the sweep's normalisation.  It is
     // taken afresh for every sweep: a Pipeline raises a node's pod count, and max_pods can drop that node together with its count.
-    if (evict_pref(S, P)) { g->pmax = 0u; post(1u); }
+    // inter-pod weight list: clear dom_sum, fill it, reduce min / max (and pmax in the same pass) — three commands.
+    if (evict_aff(S, P)) { post(2u); post(3u); g->amin = 0ll; g->amax = 0ll; g->pmax = 0u; post(4u); }
+    else if (evict_pref(S, P)) { g->pmax = 0u; post(1u); }
     g->red = 0ull;
     post(0u);
     return *((volatile unsigned long long*)&g->red);
@@ -85,18 +109,23 @@ evict_kernel(const __grid_constant__ DevSession S, const __grid_constant__ Evict
   __shared__ ClassRec s_cls;
   __shared__ Preemptor s_pre;
   __shared__ ClassPref s_pref;                     // preferred node-affinity terms of class s_pref_cls
+  __shared__ ClassAff s_aff;                       // inter-pod weight list record of class s_aff_cls
   __shared__ uint64_t s_red[EVICT_THREADS / 32];
-  __shared__ uint32_t s_cmd, s_err, s_pass, s_pmax, s_pref_cls;
+  __shared__ long long s_mn[EVICT_THREADS / 32], s_mx[EVICT_THREADS / 32];
+  __shared__ uint32_t s_list[EVICT_THREADS];       // pass 3: each warp's nodes that pass ssn.PredicateFn, compacted
+  __shared__ long long s_amin, s_amax;
+  __shared__ uint32_t s_cmd, s_err, s_pass, s_pmax, s_pref_cls, s_aff_cls;
   const uint32_t nw = gridDim.x - 1;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   uint32_t seen = 0;
-  if (threadIdx.x == 0) s_pref_cls = 0xFFFFFFFFu;
+  if (threadIdx.x == 0) { s_pref_cls = 0xFFFFFFFFu; s_aff_cls = 0xFFFFFFFFu; }
   for (;;) {
     if (threadIdx.x == 0) {
       uint32_t v;
       while ((v = ev_ld_acquire(&g->cmd_seq)) == seen) __nanosleep(40);
       s_cmd = v; s_err = 0;
       s_pass = *((volatile uint32_t*)&g->pass); s_pmax = *((volatile uint32_t*)&g->pmax);
+      s_amin = *((volatile long long*)&g->amin); s_amax = *((volatile long long*)&g->amax);
     }
     __syncthreads();
     const uint32_t cmd = s_cmd;
@@ -118,6 +147,67 @@ evict_kernel(const __grid_constant__ DevSession S, const __grid_constant__ Evict
       for (uint32_t i = threadIdx.x; i < sizeof(ClassPref) / 4; i += EVICT_THREADS) dst[i] = src[i];
       __syncthreads();
       if (threadIdx.x == 0) s_pref_cls = s_pre.cls;
+    }
+    const ClassAff* ca = evict_aff(S, s_pre);       // uniform across the CTA
+    if (ca && s_aff_cls != s_pre.cls) {             // 72 B, only when the class changes
+      const uint32_t* src = reinterpret_cast<const uint32_t*>(ca);
+      uint32_t* dst = reinterpret_cast<uint32_t*>(&s_aff);
+      for (uint32_t i = threadIdx.x; i < sizeof(ClassAff) / 4; i += EVICT_THREADS) dst[i] = src[i];
+      __syncthreads();
+      if (threadIdx.x == 0) s_aff_cls = s_pre.cls;
+    }
+    if (s_pass == 2u || s_pass == 3u) {
+      if (s_pass == 2u) {                          // clear the weights per domain
+        for (uint32_t i = blockIdx.x * EVICT_THREADS + threadIdx.x; i < S.aff.dom_total; i += nw * EVICT_THREADS) S.aff.dom_sum[i] = 0;
+      } else {
+        // weights per domain (aff_pass1_node) over the nodes that pass ssn.PredicateFn: each thread tests one node, the warp
+        // compacts its passing nodes and spreads (node, weight entry) pairs over the lanes — a class can weigh hundreds of kinds
+        const uint32_t wc = s_aff.w_cnt;
+        uint32_t* list = s_list + warp * 32;
+        auto add = [&](uint32_t slot, long long v) { atomicAdd(reinterpret_cast<unsigned long long*>(&S.aff.dom_sum[slot]), (unsigned long long)v); };
+        for (uint32_t n0 = blockIdx.x * EVICT_THREADS + (uint32_t)warp * 32u; n0 < S.N; n0 += nw * EVICT_THREADS) {
+          const uint32_t n = n0 + (uint32_t)lane;
+          const bool ok = n < S.N && evict_pred_ok(S, s_cls, n);
+          const unsigned m = __ballot_sync(0xFFFFFFFFu, ok);
+          if (ok) list[__popc(m & ((1u << lane) - 1u))] = n;
+          __syncwarp();
+          const uint32_t items = (uint32_t)__popc(m) * wc;
+          for (uint32_t k = (uint32_t)lane; k < items; k += 32u) aff_pass1_node(S.aff, s_aff, S.N, list[k / wc], add, k % wc, wc);
+          __syncwarp();
+        }
+      }
+      __threadfence();
+      __syncthreads();
+      if (threadIdx.x == 0) atomicAdd(&g->arrived, 1u);
+      continue;
+    }
+    if (s_pass == 4u) {                            // min / max InterPodAffinityPriority count (+ NodeAffinityPriority max) over this CTA's nodes
+      long long mn = 0, mx = 0;
+      uint32_t pm = 0;
+      for (uint32_t n = blockIdx.x * EVICT_THREADS + threadIdx.x; n < S.N; n += nw * EVICT_THREADS) {
+        if (!evict_pred_ok(S, s_cls, n)) continue;
+        const long long c = aff_count_node(S.aff, s_aff, S.N, n);
+        mn = c < mn ? c : mn; mx = c > mx ? c : mx;
+        if (cp) { const uint32_t v = evict_pref_count(S, s_cls, s_pref, n); pm = v > pm ? v : pm; }
+      }
+      mn = ev_warp_min(mn); mx = ev_warp_max(mx);
+      pm = __reduce_max_sync(0xFFFFFFFFu, pm);
+      if (lane == 0) { s_mn[warp] = mn; s_mx[warp] = mx; s_red[warp] = pm; }
+      __syncthreads();
+      if (warp == 0) {
+        const long long a = ev_warp_min(lane < EVICT_THREADS / 32 ? s_mn[lane] : 0ll);
+        const long long b = ev_warp_max(lane < EVICT_THREADS / 32 ? s_mx[lane] : 0ll);
+        const uint32_t p = __reduce_max_sync(0xFFFFFFFFu, lane < EVICT_THREADS / 32 ? (uint32_t)s_red[lane] : 0u);
+        if (lane == 0) {
+          if (a < 0) atomicMin(&g->amin, a);       // both start at 0 (interpod_affinity.go:205-214)
+          if (b > 0) atomicMax(&g->amax, b);
+          if (p) atomicMax(&g->pmax, p);
+          __threadfence();
+          atomicAdd(&g->arrived, 1u);
+        }
+      }
+      __syncthreads();
+      continue;
     }
     if (s_pass == 1u) {                            // pass 1: max NodeAffinityPriority count over this CTA's nodes
       uint32_t m = 0;
@@ -141,10 +231,9 @@ evict_kernel(const __grid_constant__ DevSession S, const __grid_constant__ Evict
     }
     uint64_t best = 0;
     uint32_t err = 0;
-    const ClassPref* scp = cp ? &s_pref : nullptr;
-    const uint32_t pmax = s_pmax;
+    const EvictPrio pr{cp ? &s_pref : nullptr, s_pmax, ca ? &s_aff : nullptr, s_amin, s_amax};
     for (uint32_t n = blockIdx.x * EVICT_THREADS + threadIdx.x; n < S.N; n += nw * EVICT_THREADS) {
-      const uint64_t k = evict_node_key(S, E, s_pre, s_cls, scp, pmax, n, &err);
+      const uint64_t k = evict_node_key(S, E, s_pre, s_cls, pr, n, &err);
       best = k > best ? k : best;
     }
     if (err) s_err = err;

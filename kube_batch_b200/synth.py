@@ -358,6 +358,50 @@ def add_node_pref(s: Snapshot, frac: float = 0.3, seed: int = 11) -> Snapshot:
     return s
 
 
+def add_pod_pref(s: Snapshot, frac: float = 0.15, labels: int = 8, seed: int = 17) -> Snapshot:
+    """Gives `frac` of the PodGroups the soft spread many Helm charts set by default: every pod of the group carries app=<L> (L = one
+    of `labels` values) and podAntiAffinity.preferredDuringSchedulingIgnoredDuringExecution {app=<L>, topologyKey
+    kubernetes.io/hostname} with a weight w from {1, 10, 50, 100}.  Fills kb_pod_affinity (include/kbgpu.h) exactly as
+    builder.flatten_pod_affinity would for such pods (one namespace, no placed pod carries the label or terms): no counter group;
+    one pod kind per distinct (L, w), numbered in task order, unbound (a pod placed in the session keeps Spec.NodeName ""); one key
+    set (hostname: a domain per node); the weight list of a pod of (L, w) holds, per kind (L, w') in kind order, -(w + w') — its own
+    term plus the symmetric one of the other pod.  The snapshot must not carry kb_pod_affinity yet."""
+    assert s.pod_affinity is None, "add_pod_pref builds kb_pod_affinity from scratch"
+    rng = np.random.Generator(np.random.PCG64(seed))
+    T, N = s.T, s.N
+    kinds: Dict[Tuple[int, int], int] = {}
+    task_kind = np.full(max(T, 1), -1, dtype=np.int32)
+    for j in range(s.J):
+        lo, hi = int(s.job_task_off[j]), int(s.job_task_off[j + 1])
+        if hi == lo or rng.random() >= frac:
+            continue
+        lw = (int(rng.integers(0, labels)), int(rng.choice([1, 10, 50, 100])))
+        task_kind[lo:hi] = kinds.setdefault(lw, len(kinds))
+        s.task_flags[lo:hi] |= abi.KB_TASK_HAS_POD_AFFINITY
+    NK = len(kinds)
+    of_kind = list(kinds.keys())
+    wlist = [[(k, -(w + w2)) for k, (l2, w2) in enumerate(of_kind) if l2 == lab] for (lab, w) in of_kind]
+    cnt = np.array([len(wlist[k]) if k >= 0 else 0 for k in task_kind[:T]], dtype=np.int64)
+    w_off = np.concatenate([[0], np.cumsum(cnt)]).astype(np.uint32)
+    wk = [k2 for k in task_kind[:T] if k >= 0 for (k2, _) in wlist[k]]
+    wv = [v for k in task_kind[:T] if k >= 0 for (_, v) in wlist[k]]
+    s.pod_affinity = {
+        "n_keysets": 1, "n_groups": 0, "n_kinds": NK, "n_weights": len(wk), "first_unbound_node": -1,
+        "node_domain": np.arange(max(N, 1), dtype=np.int32).reshape(1, -1), "keyset_domains": np.array([N], dtype=np.uint32),
+        "group_keyset": np.zeros(1, dtype=np.uint32), "group_count0": np.zeros(1, dtype=np.int32),
+        "group_total0": np.zeros(1, dtype=np.int32), "task_forbid": np.zeros(max(T, 1), dtype=np.uint64),
+        "task_need": np.full(max(T, 1), -1, dtype=np.int32), "task_contrib": np.zeros(max(T, 1), dtype=np.uint64),
+        "task_kind": task_kind, "node_kind_count0": np.zeros((max(1, NK), max(N, 1)), dtype=np.int32),
+        "kind_unbound": np.ones(max(1, NK), dtype=np.uint8) if NK else np.zeros(1, dtype=np.uint8),
+        "task_weight_off": w_off, "weight_kind": np.array(wk or [0], dtype=np.int32),
+        "weight_keyset": np.zeros(max(1, len(wk)), dtype=np.int32), "weight_value": np.array(wv or [0], dtype=np.int64),
+    }
+    s.meta["pod_pref_tasks"] = int((task_kind[:T] >= 0).sum()) if T else 0
+    s.meta["pod_pref_kinds"] = of_kind
+    s.invalidate()
+    return s
+
+
 # ------------------------------------------------------------------------------------------------
 # small randomised sessions for property / parity tests: every feature of the path at once
 # ------------------------------------------------------------------------------------------------
