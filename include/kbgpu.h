@@ -377,6 +377,9 @@ typedef struct kb_stats {
   uint32_t evict_sweeps;    /*   node sweeps executed (identical failing sweeps of one job are skipped)              */
   uint64_t cyc_ring;        /* cycle_kernel, KB_PIPE_TIMING=1: main-warp cycles from the end of the runs to the write-back command (hot ring) */
   uint64_t cyc_plan;        /*   ... and in the planner (scan requests for the next visits)                           */
+  uint32_t pipe_builds_used;    /* cycle_kernel, KB_PIPE_TIMING=1: pools of the next visit chain built ahead and taken   */
+  uint32_t pipe_builds_missed;  /*   ... thrown away at the visit start (another class, or no usable list was there)      */
+  uint32_t pipe_builds_cancelled; /* ... thrown away because the chain went on with another run (or the cycle ended)     */
 } kb_stats;
 
 /* Replaces nothing in the reference (process start-up): binds a CUDA device, creates the stream,

@@ -265,6 +265,9 @@ class kb_stats(C.Structure):
         ("evict_sweeps", C.c_uint32),
         ("cyc_ring", C.c_uint64),
         ("cyc_plan", C.c_uint64),
+        ("pipe_builds_used", C.c_uint32),
+        ("pipe_builds_missed", C.c_uint32),
+        ("pipe_builds_cancelled", C.c_uint32),
     ]
 
 

@@ -64,6 +64,8 @@ struct Ctl {
                           // no node passes ssn.PredicateFn for the rest of the session
   unsigned long long cyc_wait;     // replayer cycles spent between posting the visit and the eval warps' results (list wait + eval)
   unsigned long long cyc_ring, cyc_plan;      // timing mode: hot-ring append + write-back command; planner
+  // timing mode: pools of the next chain built ahead and taken / not fitting the visit / dropped because the chain went on
+  uint32_t pipe_builds_used, pipe_builds_missed, pipe_builds_cancelled;
 };
 
 // ---- persistent pipeline: global mailboxes between the replayer CTA and the scanner CTAs (kb_pipe.cuh) ----

@@ -651,6 +651,7 @@ int finish_cycle(kb_engine* e, const bool backfill, const int32_t* d_ready_start
     stats->gpu_ms = ms; stats->load_ms = e->load_ms;
     stats->scans = c.scans; stats->rescans = c.rescans;
     stats->cyc_scan = c.cyc_scan; stats->cyc_merge = c.cyc_merge; stats->cyc_replay = c.cyc_replay; stats->cyc_total = c.cyc_total; stats->cyc_steps = c.cyc_steps; stats->cyc_ctl = c.cyc_ctl; stats->cyc_ring = c.cyc_ring; stats->cyc_plan = c.cyc_plan;
+    stats->pipe_builds_used = c.pipe_builds_used; stats->pipe_builds_missed = c.pipe_builds_missed; stats->pipe_builds_cancelled = c.pipe_builds_cancelled;
     stats->predictions = c.predictions; stats->mispredictions = c.mispredictions;
     stats->chain_hits = c.chain_hits;
     stats->exchange_mode = e->world == 1 ? 0u : (e->replicated ? 3u : (D.p2p ? 2u : 1u));

@@ -40,7 +40,7 @@ constexpr int PIPE_PDEPTH = 4;             // ... and the patch warps per patch 
 // 16 warps per CTA: four per scheduler (SM sub-partition, warp % 4), so ptxas may use 128 registers per thread (a 17th warp
 // would put five on one scheduler: 96 registers and spills in the step loop).
 // replayer CTA warp roles: the main warp (0) shares its scheduler only with patch warps (4, 8, 12), which run while it waits at
-// their barrier; the prep teams, the writer / planner, the shadow prefetch and the fourth patch warp sit on the other three.
+// their barrier or, as the pool builder, while it does a chain's bookkeeping; the prep teams, the writer / planner, the shadow prefetch and the fourth patch warp sit on the other three.
 // scanner CTAs: PIPE_SCAN_GROUPS scan groups of 4 warps, then the applier warp.
 constexpr int PIPE_PREP_TEAMS = 2, PIPE_PREP_TW = 4;
 constexpr int PIPE_WARPS = 16;
@@ -110,6 +110,7 @@ __device__ __forceinline__ unsigned long long lds_u64(const void* p) {
 }
 __device__ __forceinline__ void compiler_fence() { asm volatile("" ::: "memory"); }
 __device__ __forceinline__ void bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+__device__ __forceinline__ void bar_arrive(int id, int n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 
 // record held in registers (column c at r[c]); NC = tile_ncols(R, W) is a compile-time constant here
 struct RegAcc {
@@ -432,10 +433,27 @@ template <int NC>
 struct ReplaySmem {
   Ctl ctl;
   // visit descriptor (main warp -> patch warps)
-  uint32_t v_pb, v_stamp, v_npatch, v_pvalid, v_quit, v_err, v_count, v_pad;
+  uint32_t v_pb, v_stamp, v_npatch, v_pvalid, v_quit, v_err, v_count;
+  uint32_t v_buf;                              // pkey / pfi buffer of the pool being replayed (main warp; the patch warps fill it)
+  long long t_cycle0;                          // main warp: clock64 at the first visit (kept here, not in a register)
+  uint32_t v_mode;                             // at the go barrier: 0 patch the visit's list, 1 build the next chain's pool (b_*)
   uint32_t pnode[32];                          // patch entry i: node of log entry v_stamp + i (valid bit in v_pvalid: latest entry of its node)
-  uint64_t pkey[PIPE_PDEPTH][KTOP];            // patch entry i after d more placements
-  uint32_t pfi[PIPE_PDEPTH];
+  // patch entry i after d more placements; two buffers: the builder fills one while the running chain still reads the other
+  uint64_t pkey[2][PIPE_PDEPTH][KTOP];
+  uint32_t pfi[2][PIPE_PDEPTH];
+  // pool builder (the patch warps in mode 1): the pool of the next visit chain, built while the main warp finishes this one.
+  // Descriptor (main -> builder, written before the go barrier): predicted class, class of this chain, log head after this
+  // chain's append, this chain's prepared list (slot of pb, its stamp), pkey buffer to fill, and per main-warp lane its
+  // candidate's node and slot | placements << 8 (0 placements: unmodified).
+  uint32_t b_gen, b_cls, b_ccls, b_head, b_pb, b_stamp, b_buf;
+  uint32_t b_mnode[32], b_mslot[32];
+  uint32_t b_plan;                             // volatile: command index of this chain's PCMD_PLAN once pushed (0 = not yet)
+  uint32_t b_abort;                            // volatile: the main warp will not take this pool
+  uint32_t b_ring, b_done;                     // volatile: b_gen once the hot ring holds this chain's records / once the build ended
+  uint32_t b_ok, b_seq, b_lstamp, b_npatch, b_pvalid;   // result: pool built from prepared list b_seq (stamp b_lstamp)
+  uint32_t b_urgent, b_waited;                 // result: no usable list at the first look / the prepared list was not ready yet
+  uint64_t b_key[KTOP]; uint32_t b_slot[KTOP]; uint64_t b_floor;
+  uint32_t in_use2;                            // seq + 1 of the prepared list the builder holds (volatile; second word of `claim`)
   uint64_t cmp_key[KTOP]; uint32_t cmp_slot[KTOP];       // compaction scratch of the main warp
   uint32_t step_rec[32];                       // a run's steps not yet written out: owner lane | fits-idle << 5
   uint64_t psort_key[KTOP]; uint32_t psort_slot[KTOP];   // patch entries' fresh keys, sorted (descending); slot = 32 + i
@@ -462,43 +480,208 @@ struct ReplaySmem {
   PrepBuf<NC> pb[PIPE_RQ];
 };
 
+// newest request for class `cls` in the requested table (whole warp): found; seq / stamp by reference
+template <int NC>
+__device__ __forceinline__ bool rq_find(const ReplaySmem<NC>& sm, const int lane, const uint32_t cls, uint32_t& seq, uint32_t& stamp) {
+  uint4 e = make_uint4(0u, 0u, 0u, 0u);
+  if (lane < (int)PIPE_RQ) e = lds_v4(&sm.rq_ent[lane]);
+  const bool m = e.y != 0u && e.x == cls;
+  const uint32_t s1 = m ? e.y : 0u;
+  const uint32_t best = __reduce_max_sync(FULL, s1);
+  if (best == 0) return false;
+  const int src = __ffs(__ballot_sync(FULL, m && s1 == best)) - 1;
+  seq = best - 1u;
+  stamp = __shfl_sync(FULL, e.z, src);
+  return true;
+}
+
+// Patch entry `lane` of the log window [stamp, stamp + npatch) evaluated at placement depth d for class `cls` (valid: the latest
+// entry of its node) -> pkey[buf][d] / pfi[buf][d]; depth 0 also leaves the entries sorted in psort_*.
+template <int RR, int WW>
+__device__ __forceinline__ void patch_eval(const DevSession& S, ReplaySmem<2 * RR + 6 + 3 * WW>& sm, const ClassRec& cls, const uint32_t stamp,
+                                           const uint32_t npatch, const bool have, const uint32_t node, const uint32_t buf, const int d, const int lane) {
+  constexpr uint32_t R = RR, W = WW, NC = 2 * RR + 6 + 3 * WW;
+  uint64_t key = 0;
+  bool fi = false;
+  if (have) {
+    uint64_t rec[NC];
+    const uint32_t hi = (stamp + (uint32_t)lane) % PIPE_HOT;
+#pragma unroll
+    for (uint32_t c = 0; c < NC; ++c) rec[c] = sm.hot_rec[c][hi];
+    for (int k = 0; k < d; ++k) advance_rec<RR, WW>(rec, cls);
+    RegAcc acc{rec, R, W};
+    key = eval_pair<RR, WW>(S.cf, cls, acc, node, &fi);
+  }
+  sm.pkey[buf][d][lane] = key;
+  const unsigned fim = __ballot_sync(FULL, have && fi);
+  if (lane == 0) sm.pfi[buf][d] = fim;
+  if (d == 0) {
+    // sorted (descending) for the merge with the list: rank = keys greater than mine (+ equal ones — only zeros — of lower
+    // lanes), read from shared memory with broadcast loads: ~4x shorter than a 15-stage shuffle network on this critical path.
+    // Lanes from npatch on hold zeros and rank behind every valid entry, in lane order.
+    __syncwarp();
+    uint32_t rank = (uint32_t)lane;
+    if ((uint32_t)lane < npatch) {
+      rank = 0;
+      for (uint32_t l2 = 0; l2 < npatch; ++l2) {
+        const uint64_t o = sm.pkey[buf][0][l2];
+        rank += (o > key || (o == key && l2 < (uint32_t)lane)) ? 1u : 0u;
+      }
+    }
+    sm.psort_key[rank] = key; sm.psort_slot[rank] = 32u + (uint32_t)lane;
+  }
+}
+
+// the prepared list minus the nodes of the patch set (pn: lane i holds patch entry i's node, npatch of them), compacted in list
+// order: lane-owned candidates (key at depth 0, slot = list entry).  `scratch` is the calling warp's own.
+__device__ __forceinline__ void list_minus_patch(const uint64_t* list, const uint64_t* key0, const uint32_t pn, const uint32_t npatch,
+                                                 uint64_t* scratch_key, uint32_t* scratch_slot, uint64_t& cur_key, uint32_t& slot, const int lane) {
+  const uint64_t lk = list[lane];
+  const uint32_t lnode = key_node(lk);
+  bool ok = lk != 0;
+  for (uint32_t i = 0; i < npatch; ++i) { const uint32_t o = __shfl_sync(FULL, pn, (int)i); ok = ok & (o != lnode); }   // no short-circuit: every lane takes part in the shuffle
+  const uint64_t k0 = ok ? key0[lane] : 0ull;
+  const unsigned am = __ballot_sync(FULL, k0 != 0);
+  if (k0) { const uint32_t rank = (uint32_t)__popc(am & ((1u << lane) - 1u)); scratch_key[rank] = k0; scratch_slot[rank] = (uint32_t)lane; }
+  __syncwarp();
+  const bool in = (uint32_t)lane < (uint32_t)__popc(am);
+  cur_key = in ? scratch_key[lane] : 0ull;
+  slot = in ? scratch_slot[lane] : 0u;
+  __syncwarp();
+}
+
+// Pool builder: the four patch warps prepare the pool of the NEXT visit chain while the main warp writes this chain's decisions,
+// sums and control plane.  Depth-0 warp: this chain's modified candidates -> hot ring (the records the write-back command
+// publishes), a usable prepared list of the predicted class by the main warp's own rule, claimed (in_use2), then its patch set,
+// compaction, merge and floor — the pool the main warp would build at the visit start from the same list.  Every warp evaluates
+// its depth of the patch set.  The main warp takes the pool only if the visit has the predicted class and starts at b_head.
+template <int RR, int WW, int PREF>
+__device__ __forceinline__ void pipe_build(const DevSession& S, ReplaySmem<2 * RR + 6 + 3 * WW>& sm, const int d, const int lane) {
+  constexpr uint32_t NC = 2 * RR + 6 + 3 * WW;
+  const uint32_t gen = sm.b_gen, cls_id = sm.b_cls, head = sm.b_head, buf = sm.b_buf;
+  if (d == 0) {
+    // ---- this chain's modified candidates: state after their placements -> hot ring [head - nmod, head) ----
+    const uint32_t ms = sm.b_mslot[lane], depth = ms >> 8;
+    const unsigned mm = __ballot_sync(FULL, depth > 0);
+    const uint32_t base = head - (uint32_t)__popc(mm);
+    {
+      // the writer must have written back the ring entries this append overwrites
+      const long long deadline = clock64() + PIPE_DEADLINE;
+      while (head - *((volatile uint32_t*)&sm.pub_head) > PIPE_HOT - PIPE_PATCH) {
+        if (clock64() > deadline) { *((volatile uint32_t*)&sm.v_err) = 1; break; }
+        __nanosleep(20);
+      }
+    }
+    if (depth > 0) {
+      const PrepBuf<NC>& Pc = sm.pb[sm.b_pb];
+      const uint32_t sl = ms & 63u, l = sl & 31u;
+      uint64_t r[NC];
+      if ((sl >> 5) == 0) {
+#pragma unroll
+        for (uint32_t cc = 0; cc < NC; ++cc) r[cc] = Pc.rec[cc][l];
+      } else {
+        const uint32_t hi = (sm.b_stamp + l) % PIPE_HOT;
+#pragma unroll
+        for (uint32_t cc = 0; cc < NC; ++cc) r[cc] = sm.hot_rec[cc][hi];
+      }
+      for (uint32_t k = 0; k < depth; ++k) advance_rec<RR, WW>(r, Pc.cls);
+      const uint32_t hi = (base + (uint32_t)__popc(mm & ((1u << lane) - 1u))) % PIPE_HOT;
+#pragma unroll
+      for (uint32_t cc = 0; cc < NC; ++cc) sm.hot_rec[cc][hi] = r[cc];
+      sm.hot_node[hi] = sm.b_mnode[lane]; sm.hot_cnt[hi] = depth; sm.hot_cls[hi] = sm.b_ccls;
+    }
+    __syncwarp();
+    __threadfence_block();
+    if (lane == 0) *((volatile uint32_t*)&sm.b_ring) = gen;
+    // ---- which list: the rule of the main warp at a visit start (fresh_floor is 0 after a chain that did not rescan) ----
+    const bool pref_cls = PREF && S.class_pref != nullptr && S.cf.nodeorder && S.class_pref[cls_id].n != 0;
+    uint32_t seq = 0, stamp = 0, ok = 0;
+    if (lane == 0) { sm.b_urgent = 0; sm.b_waited = 0; }
+    const long long deadline = clock64() + PIPE_DEADLINE;
+    for (bool waited = false;;) {
+      bool usable = rq_find<NC>(sm, lane, cls_id, seq, stamp);
+      usable = usable && (head - stamp) <= PIPE_PATCH && (!pref_cls || stamp == head);
+      if (usable) {
+        // claim it against the planner recycling its buffer (the second word of `claim`; see `post` in the writer warp)
+        if (lane == 0) {
+          *((volatile uint32_t*)&sm.in_use2) = seq + 1;
+          __threadfence_block();
+          const uint32_t po = *((volatile uint32_t*)&sm.posting);
+          const uint4 e = lds_v4(&sm.rq_ent[seq % PIPE_RQ]);
+          if (po == seq + 1 + PIPE_RQ || e.y != seq + 1) *((volatile uint32_t*)&sm.in_use2) = 0;
+          else ok = 1;
+        }
+        ok = __shfl_sync(FULL, ok, 0);
+        break;
+      }
+      if (waited) break;
+      if (lane == 0) sm.b_urgent = 1;
+      // the planner judges the table by the same rule at this chain's PCMD_PLAN: wait until it has, look once more
+      uint32_t stop = 0;
+      if (lane == 0) {
+        for (;;) {
+          const uint32_t pl = *((volatile uint32_t*)&sm.b_plan);
+          if (pl && (int32_t)(*((volatile uint32_t*)&sm.cmd_tail) - pl) >= 0) break;
+          if (*((volatile uint32_t*)&sm.b_abort) || *((volatile uint32_t*)&sm.v_err) || clock64() > deadline) { stop = 1; break; }
+          __nanosleep(20);
+        }
+      }
+      if (__shfl_sync(FULL, stop, 0)) break;
+      waited = true;
+    }
+    if (ok) {
+      // the prep team's buffer (the main warp's wait at a visit start)
+      uint32_t stop = 0;
+      if (lane == 0) {
+        if (*((volatile uint32_t*)&sm.pb_ready[seq % PIPE_RQ]) != seq + 1) sm.b_waited = 1;
+        while (*((volatile uint32_t*)&sm.pb_ready[seq % PIPE_RQ]) != seq + 1) {
+          if (*((volatile uint32_t*)&sm.b_abort) || *((volatile uint32_t*)&sm.v_err) || clock64() > deadline) { stop = 1; break; }
+          __nanosleep(20);
+        }
+        if (*((volatile uint32_t*)&sm.b_abort)) stop = 1;      // dropped meanwhile: no evaluation
+      }
+      if (__shfl_sync(FULL, stop, 0)) { ok = 0; if (lane == 0) *((volatile uint32_t*)&sm.in_use2) = 0; }
+    }
+    if (lane == 0) { sm.b_ok = ok; sm.b_seq = seq; sm.b_lstamp = stamp; }
+    __threadfence_block();
+  }
+  bar_sync(4, PIPE_PDEPTH * 32);                 // the list (or none) is chosen
+  if (sm.b_ok) {
+    const uint32_t stamp = sm.b_lstamp, pbi = sm.b_seq % PIPE_RQ, npatch = head - stamp;
+    const PrepBuf<NC>& P = sm.pb[pbi];
+    compiler_fence();
+    uint32_t pn = 0xFFFFFFF0u - (uint32_t)lane;
+    const bool pv = (uint32_t)lane < npatch;
+    if (pv) pn = sm.hot_node[(stamp + lane) % PIPE_HOT];
+    const unsigned same = __match_any_sync(FULL, pn);
+    const bool latest = pv && (same >> (lane + 1)) == 0u;
+    patch_eval<RR, WW>(S, sm, P.cls, stamp, npatch, latest, pn, buf, d, lane);
+    if (d == 0) {
+      uint64_t cur_key; uint32_t slot;
+      list_minus_patch(P.list, P.key[0], pn, npatch, sm.b_key, sm.b_slot, cur_key, slot, lane);
+      uint64_t dropped = 0;
+      if (npatch) { __syncwarp(); warp_merge_top32_kv(cur_key, slot, sm.psort_key[lane], sm.psort_slot[lane], dropped, lane); }
+      const uint64_t f0 = P.list[KTOP - 1];
+      sm.b_key[lane] = cur_key; sm.b_slot[lane] = slot;
+      const unsigned pvalid = __ballot_sync(FULL, latest);
+      if (lane == 0) { sm.b_floor = f0 > dropped ? f0 : dropped; sm.b_npatch = npatch; sm.b_pvalid = pvalid; }
+    }
+    __threadfence_block();
+  }
+  bar_sync(4, PIPE_PDEPTH * 32);                 // every depth is in place
+  if (d == 0 && lane == 0) *((volatile uint32_t*)&sm.b_done) = gen;
+}
+
 // patch warps (one per placement depth): patch entry `lane` = the current record of a node modified since the list's stamp,
 // from the hot ring (shared memory) — the only evaluation left on the replay's critical path
-template <int RR, int WW>
+template <int RR, int WW, int PREF>
 __device__ __forceinline__ void pipe_patch_warp(const DevSession& S, ReplaySmem<2 * RR + 6 + 3 * WW>& sm, const int d, const int lane) {
-  constexpr uint32_t R = RR, W = WW, NC = 2 * RR + 6 + 3 * WW;
   for (;;) {
     bar_sync(1, (1 + PIPE_PDEPTH) * 32);         // go
     if (*((volatile uint32_t*)&sm.v_quit)) return;
-    const ClassRec& cls = sm.pb[sm.v_pb].cls;
+    if (sm.v_mode) { pipe_build<RR, WW, PREF>(S, sm, d, lane); continue; }       // the main warp does not wait for a build here
     const bool have = ((sm.v_pvalid >> lane) & 1u) != 0;
-    const uint32_t node = sm.pnode[lane];
-    uint64_t key = 0;
-    bool fi = false;
-    if (have) {
-      uint64_t rec[NC];
-      const uint32_t hi = (sm.v_stamp + (uint32_t)lane) % PIPE_HOT;
-#pragma unroll
-      for (uint32_t c = 0; c < NC; ++c) rec[c] = sm.hot_rec[c][hi];
-      for (int k = 0; k < d; ++k) advance_rec<RR, WW>(rec, cls);
-      RegAcc acc{rec, R, W};
-      key = eval_pair<RR, WW>(S.cf, cls, acc, node, &fi);
-    }
-    sm.pkey[d][lane] = key;
-    const unsigned fim = __ballot_sync(FULL, have && fi);
-    if (lane == 0) sm.pfi[d] = fim;
-    if (d == 0) {
-      // sorted (descending) for the merge with the list: rank = keys greater than mine (+ equal ones — only zeros — of lower
-      // lanes), read from shared memory with broadcast loads: ~4x shorter than a 15-stage shuffle network on this critical path
-      __syncwarp();
-      uint32_t rank = 0;
-#pragma unroll 8
-      for (int l2 = 0; l2 < 32; ++l2) {
-        const uint64_t o = sm.pkey[0][l2];
-        rank += (o > key || (o == key && l2 < lane)) ? 1u : 0u;
-      }
-      sm.psort_key[rank] = key; sm.psort_slot[rank] = 32u + (uint32_t)lane;
-    }
+    patch_eval<RR, WW>(S, sm, sm.pb[sm.v_pb].cls, sm.v_stamp, sm.v_npatch, have, sm.pnode[lane], sm.v_buf, d, lane);
     bar_sync(1, (1 + PIPE_PDEPTH) * 32);         // done
   }
 }
@@ -672,21 +855,6 @@ __device__ __forceinline__ void pipe_shadow_warp(const DevSession& S, ReplaySmem
 }
 
 // writer / planner warp: write-backs, log, requests — everything that needs a membar, off the replay's critical path
-// newest request for class `cls` in the requested table (whole warp): found; seq / stamp by reference
-template <int NC>
-__device__ __forceinline__ bool rq_find(const ReplaySmem<NC>& sm, const int lane, const uint32_t cls, uint32_t& seq, uint32_t& stamp) {
-  uint4 e = make_uint4(0u, 0u, 0u, 0u);
-  if (lane < (int)PIPE_RQ) e = lds_v4(&sm.rq_ent[lane]);
-  const bool m = e.y != 0u && e.x == cls;
-  const uint32_t s1 = m ? e.y : 0u;
-  const uint32_t best = __reduce_max_sync(FULL, s1);
-  if (best == 0) return false;
-  const int src = __ffs(__ballot_sync(FULL, m && s1 == best)) - 1;
-  seq = best - 1u;
-  stamp = __shfl_sync(FULL, e.z, src);
-  return true;
-}
-
 template <int RR, int WW, int PREF>
 __device__ __forceinline__ void pipe_writer_warp(const DevSession& S, ReplaySmem<2 * RR + 6 + 3 * WW>& sm, const int lane) {
   constexpr uint32_t R = RR, NC = 2 * RR + 6 + 3 * WW;
@@ -710,7 +878,15 @@ __device__ __forceinline__ void pipe_writer_warp(const DevSession& S, ReplaySmem
     if (lane == 0) {
       *((volatile uint32_t*)&sm.posting) = seq + 1;
       __threadfence_block();
-      if (seq >= PIPE_RQ && *((volatile uint32_t*)&sm.in_use) == seq + 1 - PIPE_RQ) { *((volatile uint32_t*)&sm.posting) = 0; ok = 0; }
+      // in_use2 before in_use: the main warp takes over the builder's claim by setting in_use, then clearing in_use2
+      const uint32_t victim = seq + 1 - PIPE_RQ;
+      bool held = false;
+      if (seq >= PIPE_RQ) {
+        held = *((volatile uint32_t*)&sm.in_use2) == victim;
+        __threadfence_block();
+        held = held || *((volatile uint32_t*)&sm.in_use) == victim;
+      }
+      if (held) { *((volatile uint32_t*)&sm.posting) = 0; ok = 0; }
       else {
         sts_v4(&sm.rq_ent[seq % PIPE_RQ], cls, seq + 1, head, 0u);
         sts_u64(&sm.rq_word[seq % PIPE_RQ], ((unsigned long long)(seq + 1) << 32) | cls);
@@ -800,12 +976,15 @@ __device__ __forceinline__ void pipe_replayer(const DevSession& S, unsigned char
     if (lane < (int)PIPE_RQ) { sm.rq_ent[lane] = make_uint4(0u, 0u, 0u, 0u); sm.pb_ready[lane] = 0; sm.rq_word[lane] = 0ull; }
     for (uint32_t i = lane; i < PIPE_CMDS; i += 32) sm.cmd[i] = make_uint4(0u, 0u, 0u, 0u);
     if (lane < PIPE_PREP_TEAMS) sm.prep_done[lane] = (uint32_t)lane;
-    if (lane == 0) { sm.cmd_tail = 0; sm.in_use = 0; sm.posting = 0; sm.n_requests = 0; sm.pub_head = 0; sm.v_quit = 0; sm.v_err = 0; sm.v_count = 0; sm.ext_slot = 0xFFFFFFFFu; }
+    if (lane == 0) {
+      sm.cmd_tail = 0; sm.in_use = 0; sm.posting = 0; sm.n_requests = 0; sm.pub_head = 0; sm.v_quit = 0; sm.v_err = 0; sm.v_count = 0; sm.ext_slot = 0xFFFFFFFFu;
+      sm.in_use2 = 0; sm.v_buf = 0; sm.b_gen = 0; sm.b_done = 0; sm.b_ring = 0;
+    }
   }
   __syncthreads();
   int role, ridx;
   pipe_role(warp, role, ridx);
-  if (role == ROLE_PATCH) { pipe_patch_warp<RR, WW>(S, sm, ridx, lane); return; }
+  if (role == ROLE_PATCH) { pipe_patch_warp<RR, WW, PREF>(S, sm, ridx, lane); return; }
   if (role == ROLE_PREP) { pipe_prep_warp<RR, WW, PREF>(S, sm, ridx / PIPE_PREP_TW, ridx % PIPE_PREP_TW, lane); return; }
   if (role == ROLE_WRITER) { pipe_writer_warp<RR, WW, PREF>(S, sm, lane); return; }
   if (role == ROLE_SHADOW) { pipe_shadow_warp<NC>(S, sm, lane); return; }
@@ -817,6 +996,10 @@ __device__ __forceinline__ void pipe_replayer(const DevSession& S, unsigned char
   uint32_t cmd_head = 0;
   uint32_t fresh_floor = 0;      // after a rescan stop: only a list requested at or after this log position will do
   bool failed = false;
+  // the latest build of the next chain's pool (its descriptor stays in sm.b_*): 0 none, B_LIVE published by the latest run and
+  // not yet taken or dropped, B_DROPPED dropped and the builder perhaps not yet out of it
+  constexpr uint32_t B_LIVE = 1, B_DROPPED = 2;
+  uint32_t b_state = 0;
   auto push_cmd = [&](uint32_t kind, uint32_t a, uint32_t b) {       // whole warp calls it
     while (cmd_head - *((volatile uint32_t*)&sm.cmd_tail) >= PIPE_CMDS) __nanosleep(20);
     if (lane == 0) sts_v4(&sm.cmd[cmd_head % PIPE_CMDS], cmd_head + 1, kind, a, b);
@@ -835,100 +1018,149 @@ __device__ __forceinline__ void pipe_replayer(const DevSession& S, unsigned char
     }
     return __shfl_sync(FULL, ok, 0) != 0;
   };
+  // drop the live build without waiting for it: the builder stops at its next look at b_abort (visit start: the pool does not fit
+  // this visit; otherwise the chain went on or the cycle ended)
+  auto drop_build = [&](const bool at_visit_start) {
+    if (lane == 0) {
+      *((volatile uint32_t*)&sm.b_abort) = 1;
+      if (timing) { if (at_visit_start) c.pipe_builds_missed += 1; else c.pipe_builds_cancelled += 1; }
+    }
+    b_state = B_DROPPED;
+  };
+  // before the patch warps, the hot ring or the descriptor are used again: wait until the builder has left a dropped build, then
+  // release the list it may have claimed
+  auto settle_build = [&]() {
+    if (b_state != B_DROPPED) return;
+    const long long deadline = clock64() + PIPE_DEADLINE;
+    while (*((volatile uint32_t*)&sm.b_done) != sm.b_gen) { if (clock64() > deadline) { failed = true; break; } __nanosleep(20); }
+    if (lane == 0) *((volatile uint32_t*)&sm.in_use2) = 0;
+    b_state = 0;
+  };
   // the first visit's list
   if (!c.done) push_cmd(PCMD_PLAN | PLAN_FORCE_BIT | ((uint32_t)c.cur_job << 3), c.cur_class, 0u);
   uint32_t plan_idx = cmd_head;       // commands pushed up to and including the latest PCMD_PLAN
 
-  const long long t_cycle0 = clock64();
+  if (lane == 0) sm.t_cycle0 = clock64();
   while (!c.done && !failed) {
     const uint32_t cls_id = c.cur_class;
     const long long t_v0 = timing ? clock64() : 0;
     if (lane == 0) { *((volatile uint32_t*)&sm.v_count) = sm.v_count + 1; dbg_put(S.dbg, 0, sm.v_count); dbg_put(S.dbg, 1, 1u); dbg_put(S.dbg, 2, cls_id); }       // wakes the shadow warp
     // ---------------- visit start: which list ----------------
     uint32_t seq = 0, stamp = 0;
-    // a class with preferred node-affinity terms: its keys are normalised by the max count over the nodes feasible AT THE STAMP,
-    // so only a list of the current table state will do (the replay then tracks the feasible max-count nodes itself)
-    const bool pref_cls = PREF && S.class_pref != nullptr && S.cf.nodeorder && S.class_pref[cls_id].n != 0;
-    // The planner judged the table by the same rule when it handled this visit's PCMD_PLAN, or will in a moment: if nothing
-    // usable is there yet, wait for it to get that far and look again.
-    for (bool waited = false;;) {
-      bool usable = rq_find<NC>(sm, lane, cls_id, seq, stamp);
-      usable = usable && (priv_head - stamp) <= PIPE_PATCH && stamp >= fresh_floor && (!pref_cls || stamp == priv_head);
-      if (usable && claim(seq)) break;
-      if (waited) push_cmd(PCMD_PLAN | PLAN_FORCE_BIT | ((uint32_t)c.cur_job << 3), cls_id, priv_head), plan_idx = cmd_head;      // its request stepped back: ask again
-      else if (lane == 0) c.pipe_urgent += 1;
-      const long long deadline = clock64() + PIPE_DEADLINE;
-      while ((int32_t)(*((volatile uint32_t*)&sm.cmd_tail) - plan_idx) < 0) {
-        if (clock64() > deadline || *((volatile uint32_t*)&sm.v_err)) { failed = true; break; }
-        __nanosleep(20);
+    uint64_t cur_key = 0, floor_key = 0;
+    uint32_t slot = 0;
+    bool built = false;
+    if (b_state == B_LIVE) {
+      // the pool the builder prepared while the previous chain ended: usable iff this visit has the predicted class and starts
+      // at the log head it was built for
+      if (cls_id == sm.b_cls && sm.b_head == priv_head) {
+        const long long deadline = clock64() + PIPE_DEADLINE;
+        while (*((volatile uint32_t*)&sm.b_done) != sm.b_gen) {
+          if (clock64() > deadline || *((volatile uint32_t*)&sm.v_err)) { failed = true; break; }
+          __nanosleep(20);          // the builder's warps share this warp's scheduler
+        }
+        if (failed) break;
+        compiler_fence();
+        built = sm.b_ok != 0;
+      }
+      if (built) {
+        b_state = 0;
+        seq = sm.b_seq; stamp = sm.b_lstamp;
+        cur_key = sm.b_key[lane]; slot = sm.b_slot[lane]; floor_key = sm.b_floor;
+        if (lane == 0) {
+          sm.v_buf = sm.b_buf;
+          *((volatile uint32_t*)&sm.in_use) = seq + 1;        // take over the builder's claim (the planner reads in_use2 first)
+          __threadfence_block();
+          *((volatile uint32_t*)&sm.in_use2) = 0;
+          const uint32_t np = sm.b_npatch;
+          if (np) { c.pipe_patched += 1; c.pipe_patch_entries += np; c.pairs_replayed += (unsigned long long)__popc(sm.b_pvalid); }
+          c.pipe_urgent += sm.b_urgent;
+          if (timing) { c.pipe_builds_used += 1; c.mispredictions += sm.b_waited; }
+        }
+        __syncwarp();
+      } else drop_build(true);
+    }
+    if (!built) {
+      // a class with preferred node-affinity terms: its keys are normalised by the max count over the nodes feasible AT THE STAMP,
+      // so only a list of the current table state will do (the replay then tracks the feasible max-count nodes itself)
+      const bool pref_cls = PREF && S.class_pref != nullptr && S.cf.nodeorder && S.class_pref[cls_id].n != 0;
+      // The planner judged the table by the same rule when it handled this visit's PCMD_PLAN, or will in a moment: if nothing
+      // usable is there yet, wait for it to get that far and look again.
+      for (bool waited = false;;) {
+        bool usable = rq_find<NC>(sm, lane, cls_id, seq, stamp);
+        usable = usable && (priv_head - stamp) <= PIPE_PATCH && stamp >= fresh_floor && (!pref_cls || stamp == priv_head);
+        if (usable && claim(seq)) break;
+        if (waited) {
+          // its request stepped back: ask again, after a dropped build has let go of the list the planner has to recycle for it
+          settle_build();
+          if (failed) break;
+          push_cmd(PCMD_PLAN | PLAN_FORCE_BIT | ((uint32_t)c.cur_job << 3), cls_id, priv_head), plan_idx = cmd_head;
+        } else if (lane == 0) c.pipe_urgent += 1;
+        const long long deadline = clock64() + PIPE_DEADLINE;
+        while ((int32_t)(*((volatile uint32_t*)&sm.cmd_tail) - plan_idx) < 0) {
+          if (clock64() > deadline || *((volatile uint32_t*)&sm.v_err)) { failed = true; break; }
+          __nanosleep(20);
+        }
+        if (failed) break;
+        waited = true;
       }
       if (failed) break;
-      waited = true;
+      const uint32_t pbi = seq % PIPE_RQ;
+      if (lane == 0) { dbg_put(S.dbg, 1, 2u); dbg_put(S.dbg, 3, seq); dbg_put(S.dbg, 4, stamp); dbg_put(S.dbg, 5, priv_head); dbg_put(S.dbg, 6, cmd_head); }
+      {
+        const long long t_b0 = clock64(), deadline = t_b0 + PIPE_DEADLINE;
+        if (timing && lane == 0 && *((volatile uint32_t*)&sm.pb_ready[pbi]) != seq + 1) c.mispredictions += 1;      // visits that waited for their list (timing mode only)
+        while (*((volatile uint32_t*)&sm.pb_ready[pbi]) != seq + 1) {
+          if (clock64() > deadline || *((volatile uint32_t*)&sm.v_err)) { failed = true; break; }
+        }
+        compiler_fence();          // pb[pbi] was stored before pb_ready by its team (fence + barrier on their side)
+        if (timing && lane == 0) c.cyc_total += (unsigned long long)(clock64() - t_b0);      // timing mode: the wait for the prepared list
+      }
+      if (failed) break;
+      const PrepBuf<NC>& P = sm.pb[pbi];
+      settle_build();
+      if (failed) break;
+      if (lane == 0) sm.v_buf ^= 1u;
+      __syncwarp();
+      // patch set: log entries [stamp, priv_head); of several entries of one node only the latest holds its current record
+      const uint32_t npatch = priv_head - stamp;
+      uint32_t pn = 0xFFFFFFF0u - (uint32_t)lane;
+      if (npatch) {
+        const bool pv = (uint32_t)lane < npatch;
+        if (pv) pn = sm.hot_node[(stamp + lane) % PIPE_HOT];
+        const unsigned same = __match_any_sync(FULL, pn);
+        const bool latest = pv && (same >> (lane + 1)) == 0u;
+        const unsigned pvalid = __ballot_sync(FULL, latest);
+        sm.pnode[lane] = pn;
+        if (lane == 0) {
+          sm.v_pb = pbi; sm.v_stamp = stamp; sm.v_npatch = npatch; sm.v_pvalid = pvalid; sm.v_mode = 0;
+          c.pipe_patched += 1; c.pipe_patch_entries += npatch; c.pairs_replayed += (unsigned long long)__popc(pvalid);
+        }
+        __syncwarp();
+        if (lane == 0) dbg_put(S.dbg, 1, 3u);
+        bar_sync(1, (1 + PIPE_PDEPTH) * 32);        // go: the patch warps evaluate depths 0..3 of the modified nodes
+      }
+      // ---------------- meanwhile: the prepared list minus the modified nodes, compacted (order is kept) ----------------
+      list_minus_patch(P.list, P.key[0], pn, npatch, sm.cmp_key, sm.cmp_slot, cur_key, slot, lane);
+      const uint64_t f0 = P.list[KTOP - 1];
+      uint64_t dropped = 0;
+      if (npatch) {
+        bar_sync(1, (1 + PIPE_PDEPTH) * 32);        // done
+        warp_merge_top32_kv(cur_key, slot, sm.psort_key[lane], sm.psort_slot[lane], dropped, lane);
+      }
+      floor_key = f0 > dropped ? f0 : dropped;
     }
-    if (failed) break;
     fresh_floor = 0;
     const uint32_t pbi = seq % PIPE_RQ;
-    if (lane == 0) { dbg_put(S.dbg, 1, 2u); dbg_put(S.dbg, 3, seq); dbg_put(S.dbg, 4, stamp); dbg_put(S.dbg, 5, priv_head); dbg_put(S.dbg, 6, cmd_head); }
-    {
-      const long long t_b0 = clock64(), deadline = t_b0 + PIPE_DEADLINE;
-      if (timing && lane == 0 && *((volatile uint32_t*)&sm.pb_ready[pbi]) != seq + 1) c.mispredictions += 1;      // visits that waited for their list (timing mode only)
-      while (*((volatile uint32_t*)&sm.pb_ready[pbi]) != seq + 1) {
-        if (clock64() > deadline || *((volatile uint32_t*)&sm.v_err)) { failed = true; break; }
-      }
-      compiler_fence();          // pb[pbi] was stored before pb_ready by its team (fence + barrier on their side)
-      if (timing && lane == 0) c.cyc_total += (unsigned long long)(clock64() - t_b0);      // timing mode: the wait for the prepared list
-    }
-    if (failed) break;
     const PrepBuf<NC>& P = sm.pb[pbi];
-    // patch set: log entries [stamp, priv_head); of several entries of one node only the latest holds its current record
-    const uint32_t npatch = priv_head - stamp;
-    uint32_t pn = 0xFFFFFFF0u - (uint32_t)lane;
-    if (npatch) {
-      const bool pv = (uint32_t)lane < npatch;
-      if (pv) pn = sm.hot_node[(stamp + lane) % PIPE_HOT];
-      const unsigned same = __match_any_sync(FULL, pn);
-      const bool latest = pv && (same >> (lane + 1)) == 0u;
-      const unsigned pvalid = __ballot_sync(FULL, latest);
-      sm.pnode[lane] = pn;
-      if (lane == 0) {
-        sm.v_pb = pbi; sm.v_stamp = stamp; sm.v_npatch = npatch; sm.v_pvalid = pvalid;
-        c.pipe_patched += 1; c.pipe_patch_entries += npatch; c.pairs_replayed += (unsigned long long)__popc(pvalid);
-      }
-      __syncwarp();
-      if (lane == 0) dbg_put(S.dbg, 1, 3u);
-      bar_sync(1, (1 + PIPE_PDEPTH) * 32);        // go: the patch warps evaluate depths 0..7 of the modified nodes
-    }
-    // ---------------- meanwhile: the prepared list minus the modified nodes, compacted (order is kept) ----------------
-    uint64_t cur_key; uint32_t slot;
-    {
-      const uint64_t lk = P.list[lane];
-      const uint32_t lnode = key_node(lk);
-      bool ok = lk != 0;
-      for (uint32_t i = 0; i < npatch; ++i) { const uint32_t o = __shfl_sync(FULL, pn, (int)i); ok = ok & (o != lnode); }   // no short-circuit: every lane takes part in the shuffle
-      const uint64_t k0 = ok ? P.key[0][lane] : 0ull;
-      const unsigned am = __ballot_sync(FULL, k0 != 0);
-      if (k0) { const uint32_t rank = (uint32_t)__popc(am & ((1u << lane) - 1u)); sm.cmp_key[rank] = k0; sm.cmp_slot[rank] = (uint32_t)lane; }
-      __syncwarp();
-      const bool in = (uint32_t)lane < (uint32_t)__popc(am);
-      cur_key = in ? sm.cmp_key[lane] : 0ull;
-      slot = in ? sm.cmp_slot[lane] : 0u;
-      __syncwarp();
-    }
-    const uint64_t f0 = P.list[KTOP - 1];
-    uint64_t dropped = 0;
-    if (npatch) {
-      bar_sync(1, (1 + PIPE_PDEPTH) * 32);        // done
-      warp_merge_top32_kv(cur_key, slot, sm.psort_key[lane], sm.psort_slot[lane], dropped, lane);
-    }
     const long long t_v1 = timing ? clock64() : 0;
     if (lane == 0) dbg_put(S.dbg, 1, 4u);
     // ---------------- pool -> 32 lane-owned candidates ----------------
-    const uint64_t floor_key = f0 > dropped ? f0 : dropped;
     const bool have = cur_key != 0;
     const uint32_t my_node = key_node(cur_key);
     const uint32_t my_h = slot >> 5, my_l = slot & 31u;
     uint32_t depth = 0;                        // placements made on MY candidate
-    bool cur_fi = have && (((my_h ? sm.pfi[0] : P.fi[0]) >> my_l) & 1u);
+    bool cur_fi = have && (((my_h ? sm.pfi[sm.v_buf][0] : P.fi[0]) >> my_l) & 1u);
     if (lane == 0) c.scans += 1;
     const uint32_t my_lim = my_h ? (uint32_t)PIPE_PDEPTH : (uint32_t)PIPE_DEPTH;      // depths evaluated up front for MY candidate
     // my candidate's base record (state at depth 0): prepared buffer or hot ring
@@ -979,8 +1211,8 @@ __device__ __forceinline__ void pipe_replayer(const DevSession& S, unsigned char
 
     // Look-ahead of MY candidate: key / fits-idle of its NEXT state, kept in registers so that the owner of a pick moves on
     // without touching memory; the refill (a shared-memory read) is off the loop's dependency chain.
-    const uint64_t* my_chain = my_h ? &sm.pkey[0][my_l] : &P.key[0][my_l];      // + d * KTOP: depth d
-    const uint32_t* my_fiw = my_h ? &sm.pfi[0] : &P.fi[0];
+    const uint64_t* my_chain = my_h ? &sm.pkey[sm.v_buf][0][my_l] : &P.key[0][my_l];      // + d * KTOP: depth d
+    const uint32_t* my_fiw = my_h ? &sm.pfi[sm.v_buf][0] : &P.fi[0];
     uint64_t next_key = 0;
     bool next_fi = false, have_next = false;
     auto refill = [&]() {                      // state at depth + 1, from the chain evaluated up front or the extension buffer
@@ -1062,6 +1294,23 @@ __device__ __forceinline__ void pipe_replayer(const DevSession& S, unsigned char
       }
       const long long t_loop1 = timing ? clock64() : 0;
       __syncwarp();
+      // this run may end the chain: the builder starts on the next chain's pool now, the bookkeeping below runs meanwhile.  The
+      // class of the next chain is the planner's prediction (ord_chain, the queue's static job order); with several queues the
+      // queue heap reorders the visits, the prediction mostly misses and a build would only take issue slots from this warp
+      const uint32_t nxt = S.Q == 1 ? __shfl_sync(FULL, lane == 0 ? S.ord_chain[(size_t)pos0 * (KB_CHAIN_MAX - 1)] : 0u, 0) : 0xFFFFFFFFu;
+      if (reason != STOP_RESCAN && !(PREF && pref_stale) && nxt != 0xFFFFFFFFu) {
+        settle_build();
+        const unsigned mm = __ballot_sync(FULL, depth > 0);
+        sm.b_mnode[lane] = my_node; sm.b_mslot[lane] = depth > 0 ? (slot | (depth << 8)) : 0u;
+        if (lane == 0) {
+          sm.b_gen += 1; sm.b_cls = nxt; sm.b_ccls = cls_id; sm.b_head = priv_head + (uint32_t)__popc(mm); sm.b_pb = pbi; sm.b_stamp = stamp;
+          sm.b_buf = sm.v_buf ^ 1u;
+          *((volatile uint32_t*)&sm.b_plan) = 0; *((volatile uint32_t*)&sm.b_abort) = 0; sm.v_mode = 1;
+        }
+        __syncwarp();
+        bar_arrive(1, (1 + PIPE_PDEPTH) * 32);      // go, without waiting for the builder
+        b_state = B_LIVE;
+      }
       if (flushed < placed) flush(placed);
       for (uint32_t z = 0; z < placed; ++z) { jalloc = KB_DADD(jalloc, my_rq); qalloc = KB_DADD(qalloc, my_rq); }      // AllocateFunc handlers, in order
       if (lane == 0) {
@@ -1112,6 +1361,8 @@ __device__ __forceinline__ void pipe_replayer(const DevSession& S, unsigned char
       }
       __syncwarp();
       if (reason == STOP_RESCAN) { rescanned = true; break; }
+      if (b_state == B_LIVE && !(c.done || c.cur_class != cls_id || (PREF && pref_stale))) drop_build(false);      // the chain goes on
+
     }
 
     if (lane == 0) { dbg_put(S.dbg, 1, 5u); dbg_put(S.dbg, 7, c.rescans); }
@@ -1120,7 +1371,15 @@ __device__ __forceinline__ void pipe_replayer(const DevSession& S, unsigned char
     const bool modified = depth > 0;
     const unsigned mm = __ballot_sync(FULL, modified);
     const uint32_t nmod = (uint32_t)__popc(mm);
-    if (nmod) {
+    if (nmod && b_state == B_LIVE) {
+      // the builder has put these records into the ring (pipe_build)
+      const long long deadline = clock64() + PIPE_DEADLINE;
+      while (*((volatile uint32_t*)&sm.b_ring) != sm.b_gen) {
+        if (clock64() > deadline || *((volatile uint32_t*)&sm.v_err)) { failed = true; break; }
+      }
+      compiler_fence();
+    } else if (nmod) {
+      settle_build();
       // the writer must have written back the ring entries this append overwrites
       while (priv_head + nmod - *((volatile uint32_t*)&sm.pub_head) > PIPE_HOT - PIPE_PATCH) __nanosleep(20);
       if (modified) {
@@ -1132,6 +1391,9 @@ __device__ __forceinline__ void pipe_replayer(const DevSession& S, unsigned char
         for (uint32_t cc = 0; cc < NC; ++cc) sm.hot_rec[cc][hi] = rec0[cc];
         sm.hot_node[hi] = my_node; sm.hot_cnt[hi] = depth; sm.hot_cls[hi] = cls_id;
       }
+    }
+    if (failed) break;
+    if (nmod) {
       __syncwarp();
       push_cmd(PCMD_WB, priv_head, priv_head + nmod);
       priv_head += nmod;
@@ -1140,7 +1402,10 @@ __device__ __forceinline__ void pipe_replayer(const DevSession& S, unsigned char
     if (lane == 0) *((volatile uint32_t*)&sm.in_use) = 0;          // P is not read past this point
     // the planner (writer warp) requests the lists of the next visits, stamped with the log position this visit ended at
     // (pushing this before the write-back command, with the stamp ahead of the published log, was measured slower on C3)
-    if (!c.done) { push_cmd(PCMD_PLAN | (rescanned ? PLAN_FORCE_BIT : 0u) | ((uint32_t)c.cur_job << 3), c.cur_class, priv_head); plan_idx = cmd_head; }
+    if (!c.done) {
+      push_cmd(PCMD_PLAN | (rescanned ? PLAN_FORCE_BIT : 0u) | ((uint32_t)c.cur_job << 3), c.cur_class, priv_head); plan_idx = cmd_head;
+      if (b_state == B_LIVE && lane == 0) *((volatile uint32_t*)&sm.b_plan) = plan_idx;
+    }
     const long long t_r1 = timing ? clock64() : 0;
     if (lane == 0) dbg_put(S.dbg, 1, 6u);
     if (lane == 0 && timing) {
@@ -1155,6 +1420,8 @@ __device__ __forceinline__ void pipe_replayer(const DevSession& S, unsigned char
 
   // ---------------- wind down ----------------
   if (lane == 0) dbg_put(S.dbg, 1, 7u);
+  if (b_state == B_LIVE) drop_build(false);
+  settle_build();
   if (lane == 0) { *((volatile uint32_t*)&sm.v_quit) = 1; }
   __syncwarp();
   bar_sync(1, (1 + PIPE_PDEPTH) * 32);           // releases the patch warps
@@ -1164,7 +1431,7 @@ __device__ __forceinline__ void pipe_replayer(const DevSession& S, unsigned char
     while (*((volatile uint32_t*)&sm.cmd_tail) != cmd_head) { if (clock64() > deadline) { failed = true; break; } __nanosleep(40); }
   }
   if (lane == 0) {
-    if (!timing) c.cyc_total += (unsigned long long)(clock64() - t_cycle0);
+    if (!timing) c.cyc_total += (unsigned long long)(clock64() - sm.t_cycle0);
     const uint32_t n_requests = *((volatile uint32_t*)&sm.n_requests);
     c.pipe_requests += n_requests; c.pairs_scanned += (unsigned long long)n_requests * S.N;
     if ((failed || *((volatile uint32_t*)&sm.v_err)) && !c.error) c.error = 3;
