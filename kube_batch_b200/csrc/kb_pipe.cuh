@@ -111,6 +111,19 @@ __device__ __forceinline__ unsigned long long lds_u64(const void* p) {
 __device__ __forceinline__ void compiler_fence() { asm volatile("" ::: "memory"); }
 __device__ __forceinline__ void bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 __device__ __forceinline__ void bar_arrive(int id, int n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+// A bounded wait of the replayer CTA: poll done() until it holds (true), or until quit() holds or PIPE_DEADLINE cycles have passed
+// (false; what that means is the caller's).  SLEEP: ns of __nanosleep between polls, 0 for a wait on the visit's critical path.
+template <int SLEEP, typename Done, typename Quit>
+__device__ __forceinline__ bool wait_until(Done done, Quit quit) {
+  const long long deadline = clock64() + PIPE_DEADLINE;
+  while (!done()) {
+    if (quit() || clock64() > deadline) return false;
+    if (SLEEP) __nanosleep(SLEEP);
+  }
+  return true;
+}
+template <int SLEEP, typename Done>
+__device__ __forceinline__ bool wait_until(Done done) { return wait_until<SLEEP>(done, [] { return false; }); }
 
 // record held in registers (column c at r[c]); NC = tile_ncols(R, W) is a compile-time constant here
 struct RegAcc {
@@ -495,6 +508,83 @@ __device__ __forceinline__ bool rq_find(const ReplaySmem<NC>& sm, const int lane
   return true;
 }
 
+// a class with preferred node-affinity terms: its keys are normalised by the max count over the nodes feasible AT THE STAMP, so
+// only a list of the current table state will do (the replay then tracks the feasible max-count nodes itself)
+template <int PREF>
+__device__ __forceinline__ bool pref_class(const DevSession& S, const uint32_t cls) {
+  return PREF && S.class_pref != nullptr && S.cf.nodeorder && S.class_pref[cls].n != 0;
+}
+// may a list stamped at `stamp` serve a visit that starts at log position `head`: at most age_max entries behind, requested at or
+// after fresh_floor (after a rescan stop), and for a class with preferred terms (pref) of the current table state
+__device__ __forceinline__ bool list_usable(const uint32_t head, const uint32_t stamp, const uint32_t age_max, const uint32_t fresh_floor, const bool pref) {
+  return (head - stamp) <= age_max && stamp >= fresh_floor && (!pref || stamp == head);
+}
+
+// Claim prepared list `seq` against the planner recycling its buffer (whole warp): `word` is in_use (the main warp's visit) or
+// in_use2 (the pool builder).  One side of the handshake with `post` in the writer warp: store the word, fence, then read posting
+// and the table entry.  false: the planner is recycling the buffer, the word is cleared again.
+template <int NC>
+__device__ __forceinline__ bool claim(ReplaySmem<NC>& sm, uint32_t* word, const uint32_t seq, const int lane) {
+  uint32_t ok = 1;
+  if (lane == 0) {
+    *((volatile uint32_t*)word) = seq + 1;
+    __threadfence_block();
+    const uint32_t po = *((volatile uint32_t*)&sm.posting);
+    const uint4 e = lds_v4(&sm.rq_ent[seq % PIPE_RQ]);
+    if (po == seq + 1 + PIPE_RQ || e.y != seq + 1) { *((volatile uint32_t*)word) = 0; ok = 0; }
+  }
+  return __shfl_sync(FULL, ok, 0) != 0;
+}
+
+// Patch set of a list stamped at `stamp`: log entries [stamp, stamp + npatch), entry i in lane i.  pn: its node (lanes from npatch
+// on hold distinct fillers); returns whether it is the latest entry of its node, the only one that holds the node's current record.
+template <int NC>
+__device__ __forceinline__ bool patch_set(const ReplaySmem<NC>& sm, const uint32_t stamp, const uint32_t npatch, uint32_t& pn, const int lane) {
+  pn = 0xFFFFFFF0u - (uint32_t)lane;
+  const bool pv = (uint32_t)lane < npatch;
+  if (pv) pn = sm.hot_node[(stamp + lane) % PIPE_HOT];
+  const unsigned same = __match_any_sync(FULL, pn);
+  return pv && (same >> (lane + 1)) == 0u;
+}
+
+// record (state at depth 0) of pool slot `slot` of a pool built from prepared list P and the patch set at `stamp`: list entry
+// slot < 32 from the prepared buffer, patch entry slot - 32 from the hot ring
+template <int NC>
+__device__ __forceinline__ void pool_rec(const ReplaySmem<NC>& sm, const PrepBuf<NC>& P, const uint32_t stamp, const uint32_t slot, uint64_t* r) {
+  const uint32_t l = slot & 31u;
+  if ((slot >> 5) == 0) {
+#pragma unroll
+    for (uint32_t cc = 0; cc < NC; ++cc) r[cc] = P.rec[cc][l];
+  } else {
+    const uint32_t hi = (stamp + l) % PIPE_HOT;
+#pragma unroll
+    for (uint32_t cc = 0; cc < NC; ++cc) r[cc] = sm.hot_rec[cc][hi];
+  }
+}
+
+// Ring append at the end of a visit chain: each candidate with placements (depth > 0; pool slot `slot`, node `node`) -> its state
+// after them into the hot ring, in lane order, as the log entries that end at `head`.  First waits until the writer has written
+// back the ring entries this overwrites; false: that wait timed out (the records are still written).
+template <int RR, int WW>
+__device__ __forceinline__ bool ring_append(ReplaySmem<2 * RR + 6 + 3 * WW>& sm, const PrepBuf<2 * RR + 6 + 3 * WW>& P, const uint32_t stamp,
+                                            const uint32_t head, const uint32_t slot, const uint32_t depth, const uint32_t node,
+                                            const uint32_t cls_id, const int lane) {
+  constexpr uint32_t NC = 2 * RR + 6 + 3 * WW;
+  const unsigned mm = __ballot_sync(FULL, depth > 0);
+  const bool in_time = wait_until<20>([&] { return head - *((volatile uint32_t*)&sm.pub_head) <= PIPE_HOT - PIPE_PATCH; });
+  if (depth > 0) {
+    uint64_t r[NC];
+    pool_rec(sm, P, stamp, slot, r);
+    for (uint32_t k = 0; k < depth; ++k) advance_rec<RR, WW>(r, P.cls);
+    const uint32_t base = head - (uint32_t)__popc(mm);
+    const uint32_t hi = (base + (uint32_t)__popc(mm & ((1u << lane) - 1u))) % PIPE_HOT;
+#pragma unroll
+    for (uint32_t cc = 0; cc < NC; ++cc) sm.hot_rec[cc][hi] = r[cc];
+    sm.hot_node[hi] = node; sm.hot_cnt[hi] = depth; sm.hot_cls[hi] = cls_id;
+  }
+  return in_time;
+}
+
 // Patch entry `lane` of the log window [stamp, stamp + npatch) evaluated at placement depth d for class `cls` (valid: the latest
 // entry of its node) -> pkey[buf][d] / pfi[buf][d]; depth 0 also leaves the entries sorted in psort_*.
 template <int RR, int WW>
@@ -550,81 +640,58 @@ __device__ __forceinline__ void list_minus_patch(const uint64_t* list, const uin
   __syncwarp();
 }
 
+// The pool of a visit from prepared list P and its patch set (pn, npatch; see list_minus_patch): lane-owned candidates (cur_key,
+// slot), the list's compacted entries merged with the patch entries' sorted depth-0 keys (psort_*, in place once wait_patch() has
+// returned).  Returns the floor: the list's 32nd key, or the best key the merge dropped if that is higher.
+template <int NC, typename WaitPatch>
+__device__ __forceinline__ uint64_t pool_complete(const ReplaySmem<NC>& sm, const PrepBuf<NC>& P, const uint32_t pn, const uint32_t npatch,
+                                                  uint64_t* scratch_key, uint32_t* scratch_slot, uint64_t& cur_key, uint32_t& slot,
+                                                  const int lane, WaitPatch wait_patch) {
+  list_minus_patch(P.list, P.key[0], pn, npatch, scratch_key, scratch_slot, cur_key, slot, lane);
+  const uint64_t f0 = P.list[KTOP - 1];
+  uint64_t dropped = 0;
+  if (npatch) {
+    wait_patch();
+    warp_merge_top32_kv(cur_key, slot, sm.psort_key[lane], sm.psort_slot[lane], dropped, lane);
+  }
+  return f0 > dropped ? f0 : dropped;
+}
+
 // Pool builder: the four patch warps prepare the pool of the NEXT visit chain while the main warp writes this chain's decisions,
-// sums and control plane.  Depth-0 warp: this chain's modified candidates -> hot ring (the records the write-back command
-// publishes), a usable prepared list of the predicted class by the main warp's own rule, claimed (in_use2), then its patch set,
-// compaction, merge and floor — the pool the main warp would build at the visit start from the same list.  Every warp evaluates
-// its depth of the patch set.  The main warp takes the pool only if the visit has the predicted class and starts at b_head.
+// sums and control plane.  Depth-0 warp: this chain's modified candidates -> hot ring (ring_append: the records the write-back
+// command publishes), a usable prepared list of the predicted class (pref_class, list_usable: the rule of the main warp and the
+// planner), claimed with in_use2, then the pool (patch_set, pool_complete) the main warp would build at the visit start from the
+// same list.  Every warp evaluates its depth of the patch set.  The main warp takes the pool only if the visit has the predicted
+// class and starts at b_head.
 template <int RR, int WW, int PREF>
 __device__ __forceinline__ void pipe_build(const DevSession& S, ReplaySmem<2 * RR + 6 + 3 * WW>& sm, const int d, const int lane) {
   constexpr uint32_t NC = 2 * RR + 6 + 3 * WW;
   const uint32_t gen = sm.b_gen, cls_id = sm.b_cls, head = sm.b_head, buf = sm.b_buf;
   if (d == 0) {
-    // ---- this chain's modified candidates: state after their placements -> hot ring [head - nmod, head) ----
-    const uint32_t ms = sm.b_mslot[lane], depth = ms >> 8;
-    const unsigned mm = __ballot_sync(FULL, depth > 0);
-    const uint32_t base = head - (uint32_t)__popc(mm);
-    {
-      // the writer must have written back the ring entries this append overwrites
-      const long long deadline = clock64() + PIPE_DEADLINE;
-      while (head - *((volatile uint32_t*)&sm.pub_head) > PIPE_HOT - PIPE_PATCH) {
-        if (clock64() > deadline) { *((volatile uint32_t*)&sm.v_err) = 1; break; }
-        __nanosleep(20);
-      }
-    }
-    if (depth > 0) {
-      const PrepBuf<NC>& Pc = sm.pb[sm.b_pb];
-      const uint32_t sl = ms & 63u, l = sl & 31u;
-      uint64_t r[NC];
-      if ((sl >> 5) == 0) {
-#pragma unroll
-        for (uint32_t cc = 0; cc < NC; ++cc) r[cc] = Pc.rec[cc][l];
-      } else {
-        const uint32_t hi = (sm.b_stamp + l) % PIPE_HOT;
-#pragma unroll
-        for (uint32_t cc = 0; cc < NC; ++cc) r[cc] = sm.hot_rec[cc][hi];
-      }
-      for (uint32_t k = 0; k < depth; ++k) advance_rec<RR, WW>(r, Pc.cls);
-      const uint32_t hi = (base + (uint32_t)__popc(mm & ((1u << lane) - 1u))) % PIPE_HOT;
-#pragma unroll
-      for (uint32_t cc = 0; cc < NC; ++cc) sm.hot_rec[cc][hi] = r[cc];
-      sm.hot_node[hi] = sm.b_mnode[lane]; sm.hot_cnt[hi] = depth; sm.hot_cls[hi] = sm.b_ccls;
-    }
+    const uint32_t ms = sm.b_mslot[lane];
+    if (!ring_append<RR, WW>(sm, sm.pb[sm.b_pb], sm.b_stamp, head, ms & 63u, ms >> 8, sm.b_mnode[lane], sm.b_ccls, lane))
+      *((volatile uint32_t*)&sm.v_err) = 1;
     __syncwarp();
     __threadfence_block();
     if (lane == 0) *((volatile uint32_t*)&sm.b_ring) = gen;
-    // ---- which list: the rule of the main warp at a visit start (fresh_floor is 0 after a chain that did not rescan) ----
-    const bool pref_cls = PREF && S.class_pref != nullptr && S.cf.nodeorder && S.class_pref[cls_id].n != 0;
+    // ---- which list (fresh_floor is 0 after a chain that did not rescan) ----
+    const bool pref = pref_class<PREF>(S, cls_id);
+    auto off = [&] { return *((volatile uint32_t*)&sm.b_abort) || *((volatile uint32_t*)&sm.v_err); };    // dropped / the cycle failed
     uint32_t seq = 0, stamp = 0, ok = 0;
     if (lane == 0) { sm.b_urgent = 0; sm.b_waited = 0; }
-    const long long deadline = clock64() + PIPE_DEADLINE;
     for (bool waited = false;;) {
       bool usable = rq_find<NC>(sm, lane, cls_id, seq, stamp);
-      usable = usable && (head - stamp) <= PIPE_PATCH && (!pref_cls || stamp == head);
-      if (usable) {
-        // claim it against the planner recycling its buffer (the second word of `claim`; see `post` in the writer warp)
-        if (lane == 0) {
-          *((volatile uint32_t*)&sm.in_use2) = seq + 1;
-          __threadfence_block();
-          const uint32_t po = *((volatile uint32_t*)&sm.posting);
-          const uint4 e = lds_v4(&sm.rq_ent[seq % PIPE_RQ]);
-          if (po == seq + 1 + PIPE_RQ || e.y != seq + 1) *((volatile uint32_t*)&sm.in_use2) = 0;
-          else ok = 1;
-        }
-        ok = __shfl_sync(FULL, ok, 0);
-        break;
-      }
+      usable = usable && list_usable(head, stamp, PIPE_PATCH, 0u, pref);
+      if (usable) { ok = claim(sm, &sm.in_use2, seq, lane) ? 1u : 0u; break; }
       if (waited) break;
       if (lane == 0) sm.b_urgent = 1;
       // the planner judges the table by the same rule at this chain's PCMD_PLAN: wait until it has, look once more
       uint32_t stop = 0;
       if (lane == 0) {
-        for (;;) {
+        stop = !wait_until<20>([&] {
           const uint32_t pl = *((volatile uint32_t*)&sm.b_plan);
-          if (pl && (int32_t)(*((volatile uint32_t*)&sm.cmd_tail) - pl) >= 0) break;
-          if (*((volatile uint32_t*)&sm.b_abort) || *((volatile uint32_t*)&sm.v_err) || clock64() > deadline) { stop = 1; break; }
-          __nanosleep(20);
-        }
+          return pl && (int32_t)(*((volatile uint32_t*)&sm.cmd_tail) - pl) >= 0;
+        }, off);
       }
       if (__shfl_sync(FULL, stop, 0)) break;
       waited = true;
@@ -633,12 +700,9 @@ __device__ __forceinline__ void pipe_build(const DevSession& S, ReplaySmem<2 * R
       // the prep team's buffer (the main warp's wait at a visit start)
       uint32_t stop = 0;
       if (lane == 0) {
-        if (*((volatile uint32_t*)&sm.pb_ready[seq % PIPE_RQ]) != seq + 1) sm.b_waited = 1;
-        while (*((volatile uint32_t*)&sm.pb_ready[seq % PIPE_RQ]) != seq + 1) {
-          if (*((volatile uint32_t*)&sm.b_abort) || *((volatile uint32_t*)&sm.v_err) || clock64() > deadline) { stop = 1; break; }
-          __nanosleep(20);
-        }
-        if (*((volatile uint32_t*)&sm.b_abort)) stop = 1;      // dropped meanwhile: no evaluation
+        auto ready = [&] { return *((volatile uint32_t*)&sm.pb_ready[seq % PIPE_RQ]) == seq + 1; };
+        if (!ready()) sm.b_waited = 1;
+        stop = !wait_until<20>(ready, off) || *((volatile uint32_t*)&sm.b_abort);      // dropped meanwhile: no evaluation
       }
       if (__shfl_sync(FULL, stop, 0)) { ok = 0; if (lane == 0) *((volatile uint32_t*)&sm.in_use2) = 0; }
     }
@@ -650,21 +714,15 @@ __device__ __forceinline__ void pipe_build(const DevSession& S, ReplaySmem<2 * R
     const uint32_t stamp = sm.b_lstamp, pbi = sm.b_seq % PIPE_RQ, npatch = head - stamp;
     const PrepBuf<NC>& P = sm.pb[pbi];
     compiler_fence();
-    uint32_t pn = 0xFFFFFFF0u - (uint32_t)lane;
-    const bool pv = (uint32_t)lane < npatch;
-    if (pv) pn = sm.hot_node[(stamp + lane) % PIPE_HOT];
-    const unsigned same = __match_any_sync(FULL, pn);
-    const bool latest = pv && (same >> (lane + 1)) == 0u;
+    uint32_t pn;
+    const bool latest = patch_set(sm, stamp, npatch, pn, lane);
     patch_eval<RR, WW>(S, sm, P.cls, stamp, npatch, latest, pn, buf, d, lane);
     if (d == 0) {
       uint64_t cur_key; uint32_t slot;
-      list_minus_patch(P.list, P.key[0], pn, npatch, sm.b_key, sm.b_slot, cur_key, slot, lane);
-      uint64_t dropped = 0;
-      if (npatch) { __syncwarp(); warp_merge_top32_kv(cur_key, slot, sm.psort_key[lane], sm.psort_slot[lane], dropped, lane); }
-      const uint64_t f0 = P.list[KTOP - 1];
+      const uint64_t floor_key = pool_complete(sm, P, pn, npatch, sm.b_key, sm.b_slot, cur_key, slot, lane, [] { __syncwarp(); });
       sm.b_key[lane] = cur_key; sm.b_slot[lane] = slot;
       const unsigned pvalid = __ballot_sync(FULL, latest);
-      if (lane == 0) { sm.b_floor = f0 > dropped ? f0 : dropped; sm.b_npatch = npatch; sm.b_pvalid = pvalid; }
+      if (lane == 0) { sm.b_floor = floor_key; sm.b_npatch = npatch; sm.b_pvalid = pvalid; }
     }
     __threadfence_block();
   }
@@ -740,12 +798,11 @@ __device__ __forceinline__ void pipe_prep_warp(const DevSession& S, ReplaySmem<2
         P.is_pref = isp ? 1u : 0u; P.pmax = 0; P.pnmax = 0;
         if (isp) {          // written before the list words (fence in between): present once the list is
           unsigned long long a = 0, b = 0;
-          const long long deadline = clock64() + PIPE_DEADLINE;
-          for (;;) {
-            ld_relaxed_2u64(&pg->pref[slot][0], a, b);
-            if ((uint32_t)(a >> 32) == tag && (uint32_t)(b >> 32) == tag) break;
-            if (clock64() > deadline) { status = 2; break; }
-          }
+          if (!wait_until<0>([&] {
+                ld_relaxed_2u64(&pg->pref[slot][0], a, b);
+                return (uint32_t)(a >> 32) == tag && (uint32_t)(b >> 32) == tag;
+              }))
+            status = 2;
           P.pmax = (uint32_t)a; P.pnmax = (uint32_t)b;
         }
         sm.prep_status[team] = status; if (status == 2) sm.v_err = 1;
@@ -867,12 +924,9 @@ __device__ __forceinline__ void pipe_writer_warp(const DevSession& S, ReplaySmem
   // so at least one of them sees the other and steps back; a request that steps back is simply not made (a later plan repeats it).
   auto post = [&](const uint32_t cls, const uint32_t head) {
     const uint32_t seq = next_seq;
-    if (seq >= PIPE_RQ) {
-      const long long deadline = clock64() + PIPE_DEADLINE;
-      while ((int32_t)(*((volatile uint32_t*)&sm.prep_done[seq % PIPE_PREP_TEAMS]) - (seq - PIPE_RQ)) <= 0) {
-        if (clock64() > deadline) { *((volatile uint32_t*)&sm.v_err) = 1; return; }
-        __nanosleep(20);
-      }
+    if (seq >= PIPE_RQ && !wait_until<20>([&] { return (int32_t)(*((volatile uint32_t*)&sm.prep_done[seq % PIPE_PREP_TEAMS]) - (seq - PIPE_RQ)) > 0; })) {
+      *((volatile uint32_t*)&sm.v_err) = 1;
+      return;
     }
     uint32_t ok = 1;
     if (lane == 0) {
@@ -946,12 +1000,9 @@ __device__ __forceinline__ void pipe_writer_warp(const DevSession& S, ReplaySmem
         if (amax == 255u) continue;
         uint32_t s2 = 0, st2 = 0;
         const bool f = rq_find<NC>(sm, lane, pcls, s2, st2);
-        if (PREF && S.class_pref != nullptr && S.cf.nodeorder && S.class_pref[pcls].n != 0) {
-          // preferred terms: only a list of the table state at its use will do — request the next visit's now, nothing further ahead
-          if (k == 0 && !(f && st2 == head)) post(pcls, head);
-          continue;
-        }
-        if (!(f && head - st2 <= amax)) post(pcls, head);
+        const bool pref = pref_class<PREF>(S, pcls);
+        if (pref && k != 0) continue;      // only a list of the table state at its use will do: nothing further ahead
+        if (!(f && list_usable(head, st2, amax, 0u, pref))) post(pcls, head);
       }
     } else {   // PCMD_QUIT
       if (lane == 0) { st_release_u32(&pg->quit, 1u); sm.n_requests = next_seq; __threadfence_block(); *((volatile uint32_t*)&sm.cmd_tail) = tail + 1; }
@@ -1006,18 +1057,7 @@ __device__ __forceinline__ void pipe_replayer(const DevSession& S, unsigned char
     cmd_head += 1;
   };
   const bool timing = (S.pipe_pad & 1u) != 0;       // KB_PIPE_TIMING=1: clock64 phase timers of the main warp (kb_stats.cyc_*)
-  // claim prepared list `seq` for this visit against the planner recycling its buffer (see `post` in the writer warp)
-  auto claim = [&](const uint32_t seq) -> bool {
-    uint32_t ok = 1;
-    if (lane == 0) {
-      *((volatile uint32_t*)&sm.in_use) = seq + 1;
-      __threadfence_block();
-      const uint32_t po = *((volatile uint32_t*)&sm.posting);
-      const uint4 e = lds_v4(&sm.rq_ent[seq % PIPE_RQ]);
-      if (po == seq + 1 + PIPE_RQ || e.y != seq + 1) { *((volatile uint32_t*)&sm.in_use) = 0; ok = 0; }
-    }
-    return __shfl_sync(FULL, ok, 0) != 0;
-  };
+  auto err = [&] { return *((volatile uint32_t*)&sm.v_err) != 0; };      // another warp failed the cycle: a wait gives up
   // drop the live build without waiting for it: the builder stops at its next look at b_abort (visit start: the pool does not fit
   // this visit; otherwise the chain went on or the cycle ended)
   auto drop_build = [&](const bool at_visit_start) {
@@ -1031,8 +1071,7 @@ __device__ __forceinline__ void pipe_replayer(const DevSession& S, unsigned char
   // release the list it may have claimed
   auto settle_build = [&]() {
     if (b_state != B_DROPPED) return;
-    const long long deadline = clock64() + PIPE_DEADLINE;
-    while (*((volatile uint32_t*)&sm.b_done) != sm.b_gen) { if (clock64() > deadline) { failed = true; break; } __nanosleep(20); }
+    if (!wait_until<20>([&] { return *((volatile uint32_t*)&sm.b_done) == sm.b_gen; })) failed = true;
     if (lane == 0) *((volatile uint32_t*)&sm.in_use2) = 0;
     b_state = 0;
   };
@@ -1054,12 +1093,8 @@ __device__ __forceinline__ void pipe_replayer(const DevSession& S, unsigned char
       // the pool the builder prepared while the previous chain ended: usable iff this visit has the predicted class and starts
       // at the log head it was built for
       if (cls_id == sm.b_cls && sm.b_head == priv_head) {
-        const long long deadline = clock64() + PIPE_DEADLINE;
-        while (*((volatile uint32_t*)&sm.b_done) != sm.b_gen) {
-          if (clock64() > deadline || *((volatile uint32_t*)&sm.v_err)) { failed = true; break; }
-          __nanosleep(20);          // the builder's warps share this warp's scheduler
-        }
-        if (failed) break;
+        // sleeps between polls: the builder's warps share this warp's scheduler
+        if (!wait_until<20>([&] { return *((volatile uint32_t*)&sm.b_done) == sm.b_gen; }, err)) { failed = true; break; }
         compiler_fence();
         built = sm.b_ok != 0;
       }
@@ -1081,38 +1116,30 @@ __device__ __forceinline__ void pipe_replayer(const DevSession& S, unsigned char
       } else drop_build(true);
     }
     if (!built) {
-      // a class with preferred node-affinity terms: its keys are normalised by the max count over the nodes feasible AT THE STAMP,
-      // so only a list of the current table state will do (the replay then tracks the feasible max-count nodes itself)
-      const bool pref_cls = PREF && S.class_pref != nullptr && S.cf.nodeorder && S.class_pref[cls_id].n != 0;
+      const bool pref = pref_class<PREF>(S, cls_id);
       // The planner judged the table by the same rule when it handled this visit's PCMD_PLAN, or will in a moment: if nothing
       // usable is there yet, wait for it to get that far and look again.
       for (bool waited = false;;) {
         bool usable = rq_find<NC>(sm, lane, cls_id, seq, stamp);
-        usable = usable && (priv_head - stamp) <= PIPE_PATCH && stamp >= fresh_floor && (!pref_cls || stamp == priv_head);
-        if (usable && claim(seq)) break;
+        usable = usable && list_usable(priv_head, stamp, PIPE_PATCH, fresh_floor, pref);
+        if (usable && claim(sm, &sm.in_use, seq, lane)) break;
         if (waited) {
           // its request stepped back: ask again, after a dropped build has let go of the list the planner has to recycle for it
           settle_build();
           if (failed) break;
           push_cmd(PCMD_PLAN | PLAN_FORCE_BIT | ((uint32_t)c.cur_job << 3), cls_id, priv_head), plan_idx = cmd_head;
         } else if (lane == 0) c.pipe_urgent += 1;
-        const long long deadline = clock64() + PIPE_DEADLINE;
-        while ((int32_t)(*((volatile uint32_t*)&sm.cmd_tail) - plan_idx) < 0) {
-          if (clock64() > deadline || *((volatile uint32_t*)&sm.v_err)) { failed = true; break; }
-          __nanosleep(20);
-        }
-        if (failed) break;
+        if (!wait_until<20>([&] { return (int32_t)(*((volatile uint32_t*)&sm.cmd_tail) - plan_idx) >= 0; }, err)) { failed = true; break; }
         waited = true;
       }
       if (failed) break;
       const uint32_t pbi = seq % PIPE_RQ;
       if (lane == 0) { dbg_put(S.dbg, 1, 2u); dbg_put(S.dbg, 3, seq); dbg_put(S.dbg, 4, stamp); dbg_put(S.dbg, 5, priv_head); dbg_put(S.dbg, 6, cmd_head); }
       {
-        const long long t_b0 = clock64(), deadline = t_b0 + PIPE_DEADLINE;
-        if (timing && lane == 0 && *((volatile uint32_t*)&sm.pb_ready[pbi]) != seq + 1) c.mispredictions += 1;      // visits that waited for their list (timing mode only)
-        while (*((volatile uint32_t*)&sm.pb_ready[pbi]) != seq + 1) {
-          if (clock64() > deadline || *((volatile uint32_t*)&sm.v_err)) { failed = true; break; }
-        }
+        const long long t_b0 = timing ? clock64() : 0;
+        auto ready = [&] { return *((volatile uint32_t*)&sm.pb_ready[pbi]) == seq + 1; };
+        if (timing && lane == 0 && !ready()) c.mispredictions += 1;      // visits that waited for their list (timing mode only)
+        if (!wait_until<0>(ready, err)) failed = true;      // on the critical path: no sleep
         compiler_fence();          // pb[pbi] was stored before pb_ready by its team (fence + barrier on their side)
         if (timing && lane == 0) c.cyc_total += (unsigned long long)(clock64() - t_b0);      // timing mode: the wait for the prepared list
       }
@@ -1122,15 +1149,11 @@ __device__ __forceinline__ void pipe_replayer(const DevSession& S, unsigned char
       if (failed) break;
       if (lane == 0) sm.v_buf ^= 1u;
       __syncwarp();
-      // patch set: log entries [stamp, priv_head); of several entries of one node only the latest holds its current record
+      // patch set: log entries [stamp, priv_head)
       const uint32_t npatch = priv_head - stamp;
-      uint32_t pn = 0xFFFFFFF0u - (uint32_t)lane;
+      uint32_t pn = 0;
       if (npatch) {
-        const bool pv = (uint32_t)lane < npatch;
-        if (pv) pn = sm.hot_node[(stamp + lane) % PIPE_HOT];
-        const unsigned same = __match_any_sync(FULL, pn);
-        const bool latest = pv && (same >> (lane + 1)) == 0u;
-        const unsigned pvalid = __ballot_sync(FULL, latest);
+        const unsigned pvalid = __ballot_sync(FULL, patch_set(sm, stamp, npatch, pn, lane));
         sm.pnode[lane] = pn;
         if (lane == 0) {
           sm.v_pb = pbi; sm.v_stamp = stamp; sm.v_npatch = npatch; sm.v_pvalid = pvalid; sm.v_mode = 0;
@@ -1141,14 +1164,8 @@ __device__ __forceinline__ void pipe_replayer(const DevSession& S, unsigned char
         bar_sync(1, (1 + PIPE_PDEPTH) * 32);        // go: the patch warps evaluate depths 0..3 of the modified nodes
       }
       // ---------------- meanwhile: the prepared list minus the modified nodes, compacted (order is kept) ----------------
-      list_minus_patch(P.list, P.key[0], pn, npatch, sm.cmp_key, sm.cmp_slot, cur_key, slot, lane);
-      const uint64_t f0 = P.list[KTOP - 1];
-      uint64_t dropped = 0;
-      if (npatch) {
-        bar_sync(1, (1 + PIPE_PDEPTH) * 32);        // done
-        warp_merge_top32_kv(cur_key, slot, sm.psort_key[lane], sm.psort_slot[lane], dropped, lane);
-      }
-      floor_key = f0 > dropped ? f0 : dropped;
+      floor_key = pool_complete(sm, P, pn, npatch, sm.cmp_key, sm.cmp_slot, cur_key, slot, lane,
+                                [] { bar_sync(1, (1 + PIPE_PDEPTH) * 32); });      // done: the patch warps' keys are in place
     }
     fresh_floor = 0;
     const uint32_t pbi = seq % PIPE_RQ;
@@ -1163,32 +1180,11 @@ __device__ __forceinline__ void pipe_replayer(const DevSession& S, unsigned char
     bool cur_fi = have && (((my_h ? sm.pfi[sm.v_buf][0] : P.fi[0]) >> my_l) & 1u);
     if (lane == 0) c.scans += 1;
     const uint32_t my_lim = my_h ? (uint32_t)PIPE_PDEPTH : (uint32_t)PIPE_DEPTH;      // depths evaluated up front for MY candidate
-    // my candidate's base record (state at depth 0): prepared buffer or hot ring
-    auto load_rec0 = [&](uint64_t* r0) {
-      if (my_h == 0) {
-#pragma unroll
-        for (uint32_t cc = 0; cc < NC; ++cc) r0[cc] = P.rec[cc][my_l];
-      } else {
-        const uint32_t hi = (stamp + my_l) % PIPE_HOT;
-#pragma unroll
-        for (uint32_t cc = 0; cc < NC; ++cc) r0[cc] = sm.hot_rec[cc][hi];
-      }
-    };
     // extension: the whole warp evaluates depths base .. base+31 of the owner's candidate
     auto extend = [&](const uint32_t owner) {
       const uint32_t oslot = __shfl_sync(FULL, slot, owner), odepth = __shfl_sync(FULL, depth, owner), onode = __shfl_sync(FULL, my_node, owner);
       uint64_t r2[NC];
-      {
-        const uint32_t oh = oslot >> 5, ol = oslot & 31u;
-        if (oh == 0) {
-#pragma unroll
-          for (uint32_t cc = 0; cc < NC; ++cc) r2[cc] = P.rec[cc][ol];
-        } else {
-          const uint32_t hi = (stamp + ol) % PIPE_HOT;
-#pragma unroll
-          for (uint32_t cc = 0; cc < NC; ++cc) r2[cc] = sm.hot_rec[cc][hi];
-        }
-      }
+      pool_rec(sm, P, stamp, oslot, r2);
       const uint32_t base = odepth + 1, target = base + (uint32_t)lane;
       for (uint32_t k = 0; k < target; ++k) advance_rec<RR, WW>(r2, P.cls);
       RegAcc acc{r2, R, W};
@@ -1368,29 +1364,14 @@ __device__ __forceinline__ void pipe_replayer(const DevSession& S, unsigned char
     if (lane == 0) { dbg_put(S.dbg, 1, 5u); dbg_put(S.dbg, 7, c.rescans); }
     const long long t_r0 = timing ? clock64() : 0;
     // ---------------- end of the visit chain on this class: modified candidates -> hot ring + log ----------------
-    const bool modified = depth > 0;
-    const unsigned mm = __ballot_sync(FULL, modified);
-    const uint32_t nmod = (uint32_t)__popc(mm);
+    const uint32_t nmod = (uint32_t)__popc(__ballot_sync(FULL, depth > 0));
     if (nmod && b_state == B_LIVE) {
       // the builder has put these records into the ring (pipe_build)
-      const long long deadline = clock64() + PIPE_DEADLINE;
-      while (*((volatile uint32_t*)&sm.b_ring) != sm.b_gen) {
-        if (clock64() > deadline || *((volatile uint32_t*)&sm.v_err)) { failed = true; break; }
-      }
+      if (!wait_until<0>([&] { return *((volatile uint32_t*)&sm.b_ring) == sm.b_gen; }, err)) failed = true;
       compiler_fence();
     } else if (nmod) {
       settle_build();
-      // the writer must have written back the ring entries this append overwrites
-      while (priv_head + nmod - *((volatile uint32_t*)&sm.pub_head) > PIPE_HOT - PIPE_PATCH) __nanosleep(20);
-      if (modified) {
-        uint64_t rec0[NC];
-        load_rec0(rec0);
-        for (uint32_t k = 0; k < depth; ++k) advance_rec<RR, WW>(rec0, P.cls);
-        const uint32_t hi = (priv_head + (uint32_t)__popc(mm & ((1u << lane) - 1u))) % PIPE_HOT;
-#pragma unroll
-        for (uint32_t cc = 0; cc < NC; ++cc) sm.hot_rec[cc][hi] = rec0[cc];
-        sm.hot_node[hi] = my_node; sm.hot_cnt[hi] = depth; sm.hot_cls[hi] = cls_id;
-      }
+      if (!ring_append<RR, WW>(sm, P, stamp, priv_head + nmod, slot, depth, my_node, cls_id, lane)) failed = true;
     }
     if (failed) break;
     if (nmod) {
@@ -1426,10 +1407,7 @@ __device__ __forceinline__ void pipe_replayer(const DevSession& S, unsigned char
   __syncwarp();
   bar_sync(1, (1 + PIPE_PDEPTH) * 32);           // releases the patch warps
   push_cmd(PCMD_QUIT, 0, 0);
-  {
-    const long long deadline = clock64() + PIPE_DEADLINE;
-    while (*((volatile uint32_t*)&sm.cmd_tail) != cmd_head) { if (clock64() > deadline) { failed = true; break; } __nanosleep(40); }
-  }
+  if (!wait_until<40>([&] { return *((volatile uint32_t*)&sm.cmd_tail) == cmd_head; })) failed = true;
   if (lane == 0) {
     if (!timing) c.cyc_total += (unsigned long long)(clock64() - sm.t_cycle0);
     const uint32_t n_requests = *((volatile uint32_t*)&sm.n_requests);
