@@ -902,7 +902,13 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
         put(col_pods(R), (uint64_t)(uint32_t)s->node_pods[n] | ((uint64_t)(uint32_t)s->node_max_pods[n] << 32));
         // KB_SNAPSHOT_LISTED_POD_WITHOUT_NODE: InterPodAffinityMatches errors for every pair, i.e. the predicates plugin rejects
         // every node; K1 reads that as a node condition that fails (only evaluated when the plugin's predicate is enabled)
-        put(col_flags(R), (uint64_t)s->node_flags[n] | ((s->flags & KB_SNAPSHOT_LISTED_POD_WITHOUT_NODE) ? (uint64_t)KB_NODE_NOT_READY : 0ull));
+        uint64_t no_scalars = (s->node_alloc_present[n] & ~3u) == 0 ? (NODE_IDLE_NO_SCALARS | NODE_REL_NO_SCALARS) : 0ull;
+        for (uint32_t r = 2; r < R; ++r) {
+          if (s->node_idle[(size_t)r * N + n] != 0) no_scalars &= ~NODE_IDLE_NO_SCALARS;
+          if (s->node_releasing[(size_t)r * N + n] != 0) no_scalars &= ~NODE_REL_NO_SCALARS;
+        }
+        put(col_flags(R), (uint64_t)s->node_flags[n] | ((s->flags & KB_SNAPSHOT_LISTED_POD_WITHOUT_NODE) ? (uint64_t)KB_NODE_NOT_READY : 0ull) |
+                          no_scalars);
         for (uint32_t w = 0; w < W; ++w) {
           put(col_labels(R, W, w), s->node_labels[(size_t)w * N + n]);
           put(col_taints(R, W, w), s->node_taints[(size_t)w * N + n]);

@@ -182,6 +182,17 @@ KB_HD uint32_t col_flags(uint32_t R) { return 2 * R + 5; }
 KB_HD uint32_t col_labels(uint32_t R, uint32_t, uint32_t w) { return 2 * R + 6 + w; }
 KB_HD uint32_t col_taints(uint32_t R, uint32_t W, uint32_t w) { return 2 * R + 6 + W + w; }
 KB_HD uint32_t col_ports(uint32_t R, uint32_t W, uint32_t w) { return 2 * R + 6 + 2 * W + w; }
+// The flags column holds KB_NODE_* in its low 32 bits (what flags() hands to the predicates) and, above them, whether the node's
+// Idle / Releasing has no scalar map (Resource.ScalarResources == nil).  Resource.Sub leaves the scalars of such a vector alone
+// (api/resource_info.go:143-160): a task may request up to 10 milli of a scalar the node does not list (LessEqual skips it), and
+// its placement then takes nothing of that scalar.  Resource.Add of a request that names a scalar creates the map (:127-139).
+// At load a vector has no map iff the node lists no scalar in Allocatable and every scalar of the vector is 0.
+// While a vector has no map its scalars are 0, whatever the record holds: the replay's dense updates may take them below zero,
+// which no LessEqual tells apart from 0 (a scalar request of 10 milli or less is skipped, a larger one fits neither).  TileAcc —
+// the node state the engine reports, and the evictions' view — reads them as 0; evict_apply / pipeline_apply (kb_evict.h) zero
+// them when an Add gives the vector its map.
+constexpr uint64_t NODE_IDLE_NO_SCALARS = 1ull << 32;
+constexpr uint64_t NODE_REL_NO_SCALARS = 1ull << 33;
 
 KB_HD double u64_as_double(uint64_t u) {
 #if defined(__CUDA_ARCH__)
@@ -203,8 +214,12 @@ KB_HD uint64_t double_as_u64(double d) {
 struct TileAcc {
   const uint64_t* base; uint32_t i, R, W;
   KB_HD uint64_t col(uint32_t c) const { return base[c * TILE_NODES + i]; }
-  KB_HD double idle(uint32_t r) const { return u64_as_double(col(col_idle(R, r))); }
-  KB_HD double rel(uint32_t r) const { return u64_as_double(col(col_rel(R, r))); }
+  KB_HD double idle(uint32_t r) const {          // a scalar of an Idle without a scalar map is 0 (NODE_IDLE_NO_SCALARS)
+    return (r >= 2 && (col(col_flags(R)) & NODE_IDLE_NO_SCALARS)) ? 0.0 : u64_as_double(col(col_idle(R, r)));
+  }
+  KB_HD double rel(uint32_t r) const {
+    return (r >= 2 && (col(col_flags(R)) & NODE_REL_NO_SCALARS)) ? 0.0 : u64_as_double(col(col_rel(R, r)));
+  }
   KB_HD int64_t alloc_cpu() const { return (int64_t)col(col_alloc_cpu(R)); }
   KB_HD int64_t alloc_mem() const { return (int64_t)col(col_alloc_mem(R)); }
   KB_HD int64_t nz_cpu() const { return (int64_t)col(col_nz_cpu(R)); }
@@ -216,6 +231,17 @@ struct TileAcc {
   KB_HD uint64_t taints(uint32_t w) const { return col(col_taints(R, W, w)); }
   KB_HD uint64_t ports(uint32_t w) const { return col(col_ports(R, W, w)); }
 };
+
+// Resource.Add of a request naming a scalar on node record `t` (first column, TILE_NODES apart): the vectors in `which`
+// (NODE_IDLE_NO_SCALARS / NODE_REL_NO_SCALARS) that had no scalar map get one, with every scalar at 0
+KB_HD void set_scalar_maps(uint64_t* t, const uint32_t R, const uint64_t which) {
+  uint64_t& fl = t[(size_t)col_flags(R) * TILE_NODES];
+  for (uint32_t k = 2; k < R; ++k) {
+    if (fl & which & NODE_IDLE_NO_SCALARS) t[(size_t)col_idle(R, k) * TILE_NODES] = double_as_u64(0.0);
+    if (fl & which & NODE_REL_NO_SCALARS) t[(size_t)col_rel(R, k) * TILE_NODES] = double_as_u64(0.0);
+  }
+  fl &= ~which;
+}
 
 // ---------------------------------------------------------------------------------------------
 // ordering

@@ -297,6 +297,9 @@ KB_HD void evict_apply(const DevSession& S, const EvictDev& E, const uint32_t no
     }
   } else if (!undo && (E.r_flags[slot] & KB_RUNNING_AFF_MEMBER) && E.ctl->error == 0) E.ctl->error = 3;
   S.job_ready[j] += undo ? 1 : -1;                                         // Running counts as ready, Releasing does not (job_info.go:383-393)
+  // Idle.Add and Releasing.Add of a request that names a scalar give both vectors a scalar map, starting from 0 (kb_ctl.h); after
+  // that the Sub below takes the scalars too, so the dense update is exact
+  if (E.r_present[slot] & ~3u) set_scalar_maps(t, R, NODE_IDLE_NO_SCALARS | NODE_REL_NO_SCALARS);
   for (uint32_t k = 0; k < R; ++k) {
     const double r = E.r_resreq[(size_t)k * n + slot];
     double idle = u64_as_double(t[(size_t)col_idle(R, k) * TILE_NODES]);
@@ -325,6 +328,8 @@ KB_HD void pipeline_apply(const DevSession& S, const EvictDev& E, const Preempto
   const size_t tile_u64 = (size_t)S.ncols * TILE_NODES;
   uint64_t* t = S.tiles + (size_t)(node / TILE_NODES) * tile_u64 + (node % TILE_NODES);
   E.job_waiting[j] += undo ? -1 : 1;
+  // Statement.unpipeline's Releasing.Add of a request naming a scalar gives Releasing its scalar map, starting from 0 (kb_ctl.h)
+  if (undo && (E.task_present[P.task] & ~3u)) set_scalar_maps(t, R, NODE_REL_NO_SCALARS);
   for (uint32_t k = 0; k < R; ++k) {
     const double r = c.resreq[k];
     double rel = u64_as_double(t[(size_t)col_rel(R, k) * TILE_NODES]);
