@@ -49,9 +49,14 @@ var actionID = map[string]C.uint8_t{"reclaim": C.KB_ACT_RECLAIM, "allocate": C.K
 
 // NewCycle: `actions` must be the scheduler configuration's action list restricted to the four built-ins, in order.
 func NewCycle(e *Engine, actions []string) (*Cycle, error) {
-	for _, a := range actions {
+	for i, a := range actions {
 		if _, ok := actionID[a]; !ok {
 			return nil, fmt.Errorf("kbgpu: unknown action %q", a)
+		}
+		for _, prev := range actions[:i] {
+			if prev == a { // replay finds an action's slice of the result by its name
+				return nil, fmt.Errorf("kbgpu: action %q is listed twice", a)
+			}
 		}
 	}
 	return &Cycle{engine: e, actions: actions}, nil
@@ -82,7 +87,9 @@ func (c *Cycle) flattenRunning(ssn *framework.Session, f *Flat) *runningFlat {
 			if _, ok := jidx[t.Job]; !ok { // reclaim.go:131: tasks of unknown jobs are never candidates
 				continue
 			}
-			c.running = append(c.running, t)
+			// reclaim.go:135-136: a clone, so that the node's own copy still holds Running when ssn.Evict / Statement.Evict
+			// take it off the node (node_info.go:217-245); evicting the node's copy itself would leave Releasing unchanged
+			c.running = append(c.running, t.Clone())
 			nodeOf = append(nodeOf, uint32(ni))
 		}
 	}

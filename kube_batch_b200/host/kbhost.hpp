@@ -1,14 +1,15 @@
-// kbhost.hpp — C++17 host-side mirror of the kube-batch interface around the allocate path, sitting ABOVE the
+// kbhost.hpp — C++17 host-side mirror of the kube-batch interface around the scheduling actions, sitting ABOVE the
 // C ABI of libkbgpu.so (include/kbgpu.h).  The reference is Go and no Go toolchain exists in this image, so this
 // header plays the role the Go shim (go/kbgpu) plays inside kube-batch: same names, same argument meaning, same
-// error behaviour, so tests can be written like pkg/scheduler/actions/allocate/allocate_test.go.
+// error behaviour, so tests can be written like pkg/scheduler/actions/{allocate,preempt,reclaim}/*_test.go.
 //
 //   kb::api        Resource, TaskInfo, NodeInfo, JobInfo, QueueInfo, TaskStatus      (pkg/scheduler/api)
 //   kb::conf       PluginOption, Tier                                                 (pkg/scheduler/conf)
-//   kb::cache      SchedulerCache{AddNode,AddPod,AddPodGroup,AddQueue,Snapshot}, Binder (pkg/scheduler/cache)
-//   kb::framework  Session, Plugin, Action, Arguments, RegisterPluginBuilder, OpenSession, CloseSession
+//   kb::cache      SchedulerCache{AddNode,AddPod,AddPodGroup,AddQueue,Snapshot,Evict}, Binder, Evictor (pkg/scheduler/cache)
+//   kb::framework  Session, Statement, Plugin, Action, Arguments, RegisterPluginBuilder, OpenSession, CloseSession
 //   kb::plugins    the built-in plugin builders by name                                (pkg/scheduler/plugins/factory.go)
 //   kb::actions::allocate::New()->Execute(ssn)                                         (pkg/scheduler/actions/allocate)
+//   kb::actions::cycle::Cycle  the whole action list as ONE kb_cycle, replayed by four action shells (go/kbgpu/cycle.go)
 //
 // What differs from the reference, by construction: plugin callbacks are arbitrary Go closures there; a GPU engine
 // can only honour the BUILT-IN ones.  Session::Add*Fn therefore registers a *descriptor* (which built-in function,
@@ -84,6 +85,7 @@ struct Pod {                                          // the v1.Pod fields the p
   struct HostPort { std::string HostIP, Protocol; int Port; };
   std::vector<HostPort> HostPorts;
   int32_t Priority = 1;
+  std::string PriorityClassName;                      // Spec.PriorityClassName (conformance.go:45-53)
   int64_t CreationTimestamp = 0;
   bool Deleting = false;
 };
@@ -103,6 +105,7 @@ struct TaskInfo {                                     // api/job_info.go:36-54
   int Status = Pending;
   int32_t Priority = 1;
   std::shared_ptr<Pod> pod;
+  std::shared_ptr<TaskInfo> Clone() const { return std::make_shared<TaskInfo>(*this); }   // job_info.go:96-113 (the Pod is shared)
 };
 
 struct NodeInfo {                                     // api/node_info.go:28-47
@@ -110,7 +113,8 @@ struct NodeInfo {                                     // api/node_info.go:28-47
   std::shared_ptr<Node> node;
   Resource Releasing, Idle, Used, Allocatable;
   std::map<std::string, std::shared_ptr<TaskInfo>> Tasks;
-  // api/node_info.go:172-212
+  // api/node_info.go:172-212.  The node keeps its own copy of the task, so a later status change of the caller's object
+  // leaves the node's resources alone until UpdateTask / RemoveTask.
   void AddTask(const std::shared_ptr<TaskInfo>& task) {
     if (Tasks.count(task->Namespace + "/" + task->Name)) throw std::runtime_error("task already on node " + Name);
     switch (task->Status) {
@@ -120,8 +124,23 @@ struct NodeInfo {                                     // api/node_info.go:28-47
     }
     Used.Add(task->Resreq);
     task->NodeName = Name;
-    Tasks[task->Namespace + "/" + task->Name] = task;
+    Tasks[task->Namespace + "/" + task->Name] = task->Clone();
   }
+  // api/node_info.go:214-245: gives back what the node's own copy holds, by that copy's status
+  void RemoveTask(const TaskInfo& ti) {
+    auto it = Tasks.find(ti.Namespace + "/" + ti.Name);
+    if (it == Tasks.end()) throw std::runtime_error("failed to find task " + ti.Namespace + "/" + ti.Name + " on host " + Name);
+    const TaskInfo& task = *it->second;
+    switch (task.Status) {
+      case Releasing_: Releasing.SubUnchecked(task.Resreq); Idle.Add(task.Resreq); break;
+      case Pipelined: Releasing.Add(task.Resreq); break;
+      default: Idle.Add(task.Resreq); break;
+    }
+    Used.SubUnchecked(task.Resreq);
+    Tasks.erase(it);
+  }
+  // api/node_info.go:245-259
+  void UpdateTask(const std::shared_ptr<TaskInfo>& ti) { RemoveTask(*ti); AddTask(ti); }
   static constexpr int Releasing_ = api::Releasing;
 };
 
@@ -133,12 +152,19 @@ struct JobInfo {                                      // api/job_info.go:127-154
   std::map<int, std::map<std::string, std::shared_ptr<TaskInfo>>> TaskStatusIndex;
   Resource Allocated;
   void AddTaskInfo(const std::shared_ptr<TaskInfo>& t) { Tasks[t->UID] = t; TaskStatusIndex[t->Status][t->UID] = t; if (AllocatedStatus(t->Status)) Allocated.Add(t->Resreq); }
-  void UpdateTaskStatus(const std::shared_ptr<TaskInfo>& t, int status) {   // job_info.go:247-264
-    auto it = TaskStatusIndex.find(t->Status);
-    if (it != TaskStatusIndex.end()) { if (AllocatedStatus(t->Status)) Allocated.SubUnchecked(t->Resreq); it->second.erase(t->UID); if (it->second.empty()) TaskStatusIndex.erase(it); }
+  // job_info.go:247-264: the job's entry for the UID (found by UID, removed by ITS status) is replaced by `t` — which may be
+  // another object for the same task, e.g. the clone of a node's copy that reclaim / preempt evict
+  void UpdateTaskStatus(const std::shared_ptr<TaskInfo>& t, int status) {
+    auto found = Tasks.find(t->UID);
+    if (found != Tasks.end()) {                         // DeleteTaskInfo, job_info.go:279-295
+      const std::shared_ptr<TaskInfo> old = found->second;
+      if (AllocatedStatus(old->Status)) Allocated.SubUnchecked(old->Resreq);
+      Tasks.erase(found);
+      auto it = TaskStatusIndex.find(old->Status);
+      if (it != TaskStatusIndex.end()) { it->second.erase(old->UID); if (it->second.empty()) TaskStatusIndex.erase(it); }
+    }
     t->Status = status;
-    TaskStatusIndex[status][t->UID] = t;
-    if (AllocatedStatus(status)) Allocated.Add(t->Resreq);
+    AddTaskInfo(t);
   }
   int32_t ReadyTaskNum() const {                      // job_info.go:383-393
     int n = 0;
@@ -174,6 +200,11 @@ struct FakeBinder : Binder {                          // util/test_utils.go:95-1
   std::map<std::string, std::string> Binds;
   void Bind(const api::TaskInfo& task, const std::string& hostname) override { Binds[task.Namespace + "/" + task.Name] = hostname; }
 };
+struct Evictor { virtual ~Evictor() = default; virtual void Evict(const api::Pod& pod) = 0; };   // cache/interface.go:68-72
+struct FakeEvictor : Evictor {                        // util/test_utils.go:114-133
+  std::vector<std::string> Evicts;                    // in call order
+  void Evict(const api::Pod& pod) override { Evicts.push_back(pod.Namespace + "/" + pod.Name); }
+};
 struct PodGroup { std::string Namespace, Name, Queue; int32_t MinMember = 0; int32_t Priority = 0; int64_t CreationTimestamp = 0; };
 struct ClusterInfo {                                  // api/cluster_info.go:22-26
   std::map<std::string, std::shared_ptr<api::JobInfo>> Jobs;
@@ -185,6 +216,11 @@ struct SchedulerCache {                               // the literal cache of al
   std::map<std::string, std::shared_ptr<api::JobInfo>> Jobs;
   std::map<std::string, std::shared_ptr<api::QueueInfo>> Queues;
   std::shared_ptr<Binder> binder;
+  std::shared_ptr<Evictor> evictor;
+  // cache/cache.go:425-480.  The session shares this cache's objects (Snapshot does not deep-copy), so the status and node
+  // updates of the reference's cache.Evict are the session's own (Session::Evict, Statement::Evict); what is left is the
+  // call to the Evictor.
+  void Evict(const api::TaskInfo& task, const std::string& /*reason*/) { if (evictor) evictor->Evict(*task.pod); }
   void AddNode(const api::Node& n) {
     auto ni = std::make_shared<api::NodeInfo>();
     ni->Name = n.Name; ni->node = std::make_shared<api::Node>(n);
@@ -331,11 +367,65 @@ class Session {                                       // framework/session.go:37
     if (cache && cache->binder) cache->binder->Bind(*task, task->NodeName);
     Jobs.at(task->Job)->UpdateTaskStatus(task, api::Binding);
   }
+  // framework/session.go:317-353.  Callers pass a clone of the node's task (reclaim.go:135-136): the node's own copy must
+  // still hold the old status when UpdateTask takes it off the node.
+  void Evict(const std::shared_ptr<api::TaskInfo>& reclaimee, const std::string& reason) {
+    if (cache) cache->Evict(*reclaimee, reason);
+    Jobs.at(reclaimee->Job)->UpdateTaskStatus(reclaimee, api::Releasing);
+    auto node = Nodes.find(reclaimee->NodeName);
+    if (node != Nodes.end()) node->second->UpdateTask(reclaimee);
+  }
+};
+
+// framework/statement.go: evictions and pipelines applied to the session at once, sent to the cache by Commit or undone in
+// reverse order by Discard.  ssn.Statement() (session.go:186-191) is `Statement stmt(ssn)` here.
+class Statement {
+ public:
+  explicit Statement(Session* ssn) : ssn_(ssn) {}
+  void Evict(const std::shared_ptr<api::TaskInfo>& reclaimee, const std::string& reason) {   // statement.go:37-69
+    updateStatus(reclaimee, api::Releasing);
+    auto node = ssn_->Nodes.find(reclaimee->NodeName);
+    if (node != ssn_->Nodes.end()) node->second->UpdateTask(reclaimee);
+    operations_.push_back({true, reclaimee, reason});
+  }
+  void Pipeline(const std::shared_ptr<api::TaskInfo>& task, const std::string& hostname) {  // statement.go:113-152
+    updateStatus(task, api::Pipelined);
+    ssn_->Nodes.at(hostname)->AddTask(task);
+    operations_.push_back({false, task, hostname});
+  }
+  void Commit() {                                                                           // statement.go:210-221
+    for (auto& op : operations_) if (op.evict && ssn_->cache) ssn_->cache->Evict(*op.task, op.arg);
+  }
+  void Discard() {                                                                          // statement.go:196-208
+    for (auto it = operations_.rbegin(); it != operations_.rend(); ++it) {
+      auto& task = it->task;
+      if (it->evict) {                                  // unevict, statement.go:83-111
+        updateStatus(task, api::Running);
+        auto node = ssn_->Nodes.find(task->NodeName);
+        if (node != ssn_->Nodes.end()) node->second->UpdateTask(task);
+      } else {                                          // unpipeline, statement.go:157-194
+        updateStatus(task, api::Pending);
+        auto node = ssn_->Nodes.find(task->NodeName);
+        if (node != ssn_->Nodes.end()) node->second->RemoveTask(*task);
+      }
+    }
+  }
+
+ private:
+  struct operation { bool evict; std::shared_ptr<api::TaskInfo> task; std::string arg; };   // arg: reason / hostname
+  void updateStatus(const std::shared_ptr<api::TaskInfo>& task, int status) {
+    auto job = ssn_->Jobs.find(task->Job);
+    if (job != ssn_->Jobs.end()) job->second->UpdateTaskStatus(task, status);
+  }
+  Session* ssn_;
+  std::vector<operation> operations_;
 };
 
 // framework/framework.go:30-52
 inline std::unique_ptr<Session> OpenSession(cache::SchedulerCache* cache, const std::vector<conf::Tier>& tiers) {
+  static uint64_t sessions = 0;
   auto ssn = std::make_unique<Session>();
+  ssn->UID = "session-" + std::to_string(++sessions);   // uuid.NewUUID() (session.go:65): what a cycle's result is cached under
   ssn->cache = cache;
   auto snap = cache->Snapshot();
   ssn->Jobs = snap.Jobs; ssn->Nodes = snap.Nodes; ssn->Queues = snap.Queues;
@@ -385,7 +475,7 @@ namespace actions { namespace allocate {
 // Flattened session: the SoA arrays of kb_snapshot plus the back-references needed to replay decisions.
 struct Flat {
   uint32_t R = 2, W = 1, N = 0, T = 0, J = 0, Q = 0;
-  std::vector<std::string> dims, nodeNames;
+  std::vector<std::string> dims, nodeNames, jobIDs;
   std::vector<std::shared_ptr<api::TaskInfo>> tasks;
   std::vector<double> node_idle, node_releasing, node_used, node_allocatable, task_initreq, task_resreq, job_alloc0;
   std::vector<uint32_t> node_alloc_present, node_flags, task_res_present, task_n_aff, task_flags, task_uid_rank, job_task_off, job_alloc0_present, job_queue;
@@ -413,6 +503,7 @@ inline Flat Flatten(const framework::Session& ssn) {
   std::vector<std::shared_ptr<api::NodeInfo>> nodes; for (auto& kv : ssn.Nodes) nodes.push_back(kv.second);       // std::map: ascending Name
   std::vector<std::shared_ptr<api::QueueInfo>> queues; for (auto& kv : ssn.Queues) queues.push_back(kv.second);
   std::vector<std::shared_ptr<api::JobInfo>> jobs; for (auto& kv : ssn.Jobs) jobs.push_back(kv.second);          // ascending JobID
+  for (auto& j : jobs) f.jobIDs.push_back(j->UID);
   std::map<std::string, uint32_t> qidx; for (uint32_t i = 0; i < queues.size(); ++i) qidx[queues[i]->UID] = i;
   f.N = (uint32_t)nodes.size(); f.J = (uint32_t)jobs.size(); f.Q = (uint32_t)queues.size();
   // pending tasks grouped by job; UID ranks
@@ -513,17 +604,19 @@ inline Flat Flatten(const framework::Session& ssn) {
 // default list, pkg/scheduler/util.go:31-42) is two such calls, exactly like the reference runs two Execute()s on one
 // session.  (A shim that wants to save the second flatten + upload can call kb_allocate and kb_backfill back to back on
 // one loaded session instead: see INTEGRATION.md.)
-inline void ExecuteOnGpu(framework::Session* ssn, const bool backfill) {
-  {
-    // tiers: only built-in registrations can be honoured
-    std::vector<kb_plugin_option> opts; std::vector<kb_tier> tiers; std::vector<std::vector<const char*>> keys, vals;
-    size_t total = 0; for (auto& t : ssn->Tiers) total += t.Plugins.size();
+// The session's tiers as kb_plugin_conf.  Only built-in registrations can be honoured.  `conf` points into this object,
+// which therefore stays where it was built.
+struct PluginConf {
+  std::vector<kb_plugin_option> opts; std::vector<kb_tier> tiers; std::vector<std::vector<const char*>> keys, vals;
+  kb_plugin_conf conf{};
+  explicit PluginConf(const framework::Session& ssn) {
+    size_t total = 0; for (auto& t : ssn.Tiers) total += t.Plugins.size();
     opts.reserve(total); keys.reserve(total); vals.reserve(total);
-    for (auto& t : ssn->Tiers) {
+    for (auto& t : ssn.Tiers) {
       kb_tier ct{}; ct.n_plugins = (uint32_t)t.Plugins.size(); ct.plugins = opts.data() + opts.size();
       for (auto& p : t.Plugins) {
-        auto reg = ssn->registered.find(p.Name);
-        if (reg != ssn->registered.end()) for (auto b : reg->second) if (b == framework::Builtin::Foreign)
+        auto reg = ssn.registered.find(p.Name);
+        if (reg != ssn.registered.end()) for (auto b : reg->second) if (b == framework::Builtin::Foreign)
           throw std::runtime_error("plugin " + p.Name + " registered a non built-in function: the GPU path cannot honour it (no CPU fallback)");
         kb_plugin_option o{}; o.name = p.Name.c_str();
         o.enabled_job_order = p.EnabledJobOrder == 1; o.enabled_job_ready = p.EnabledJobReady == 1; o.enabled_job_pipelined = p.EnabledJobPipelined == 1;
@@ -536,41 +629,68 @@ inline void ExecuteOnGpu(framework::Session* ssn, const bool backfill) {
       }
       tiers.push_back(ct);
     }
-    kb_plugin_conf conf{(uint32_t)tiers.size(), tiers.data()};
-    Flat f = Flatten(*ssn);
-    kb_snapshot s{};
-    s.abi_version = KB_ABI_VERSION; s.R = f.R; s.W = f.W; s.N = f.N; s.T = f.T; s.J = f.J; s.Q = f.Q;
-    s.node_idle = f.node_idle.data(); s.node_releasing = f.node_releasing.data(); s.node_used = f.node_used.data(); s.node_allocatable = f.node_allocatable.data();
-    s.node_alloc_present = f.node_alloc_present.data(); s.node_alloc_cpu = f.node_alloc_cpu.data(); s.node_alloc_mem = f.node_alloc_mem.data();
-    s.node_nz_cpu = f.node_nz_cpu.data(); s.node_nz_mem = f.node_nz_mem.data(); s.node_pods = f.node_pods.data(); s.node_max_pods = f.node_max_pods.data();
-    s.node_flags = f.node_flags.data(); s.node_labels = f.node_labels.data(); s.node_taints = f.node_taints.data(); s.node_ports = f.node_ports.data();
-    s.task_initreq = f.task_initreq.data(); s.task_resreq = f.task_resreq.data(); s.task_res_present = f.task_res_present.data();
-    s.task_nz_cpu = f.task_nz_cpu.data(); s.task_nz_mem = f.task_nz_mem.data(); s.task_sel_req = f.task_sel_req.data(); s.task_aff_terms = f.task_aff.data();
-    s.task_n_aff_terms = f.task_n_aff.data(); s.task_tol = f.task_tol.data(); s.task_port_own = f.task_port_own.data(); s.task_port_conflict = f.task_port_conflict.data();
-    s.task_flags = f.task_flags.data(); s.task_prio = f.task_prio.data(); s.task_ctime = f.task_ctime.data(); s.task_uid_rank = f.task_uid_rank.data();
-    s.job_task_off = f.job_task_off.data(); s.job_min_avail = f.job_min_avail.data(); s.job_ready0 = f.job_ready0.data(); s.job_alloc0 = f.job_alloc0.data();
-    s.job_alloc0_present = f.job_alloc0_present.data(); s.job_queue = f.job_queue.data(); s.job_prio = f.job_prio.data(); s.job_ctime = f.job_ctime.data();
-    s.queue_weight = f.queue_weight.data(); s.queue_ctime = f.queue_ctime.data();
+    conf = kb_plugin_conf{(uint32_t)tiers.size(), tiers.data()};
+  }
+  PluginConf(const PluginConf&) = delete;
+  PluginConf& operator=(const PluginConf&) = delete;
+};
 
+// kb_snapshot over the arrays of `f` (which must outlive it)
+inline kb_snapshot SnapshotOf(Flat& f) {
+  kb_snapshot s{};
+  s.abi_version = KB_ABI_VERSION; s.R = f.R; s.W = f.W; s.N = f.N; s.T = f.T; s.J = f.J; s.Q = f.Q;
+  s.node_idle = f.node_idle.data(); s.node_releasing = f.node_releasing.data(); s.node_used = f.node_used.data(); s.node_allocatable = f.node_allocatable.data();
+  s.node_alloc_present = f.node_alloc_present.data(); s.node_alloc_cpu = f.node_alloc_cpu.data(); s.node_alloc_mem = f.node_alloc_mem.data();
+  s.node_nz_cpu = f.node_nz_cpu.data(); s.node_nz_mem = f.node_nz_mem.data(); s.node_pods = f.node_pods.data(); s.node_max_pods = f.node_max_pods.data();
+  s.node_flags = f.node_flags.data(); s.node_labels = f.node_labels.data(); s.node_taints = f.node_taints.data(); s.node_ports = f.node_ports.data();
+  s.task_initreq = f.task_initreq.data(); s.task_resreq = f.task_resreq.data(); s.task_res_present = f.task_res_present.data();
+  s.task_nz_cpu = f.task_nz_cpu.data(); s.task_nz_mem = f.task_nz_mem.data(); s.task_sel_req = f.task_sel_req.data(); s.task_aff_terms = f.task_aff.data();
+  s.task_n_aff_terms = f.task_n_aff.data(); s.task_tol = f.task_tol.data(); s.task_port_own = f.task_port_own.data(); s.task_port_conflict = f.task_port_conflict.data();
+  s.task_flags = f.task_flags.data(); s.task_prio = f.task_prio.data(); s.task_ctime = f.task_ctime.data(); s.task_uid_rank = f.task_uid_rank.data();
+  s.job_task_off = f.job_task_off.data(); s.job_min_avail = f.job_min_avail.data(); s.job_ready0 = f.job_ready0.data(); s.job_alloc0 = f.job_alloc0.data();
+  s.job_alloc0_present = f.job_alloc0_present.data(); s.job_queue = f.job_queue.data(); s.job_prio = f.job_prio.data(); s.job_ctime = f.job_ctime.data();
+  s.queue_weight = f.queue_weight.data(); s.queue_ctime = f.queue_ctime.data();
+  return s;
+}
+
+// A refusal of the engine: std::runtime_error with kb_last_error and the status
+inline void Check(int rc, const char* what, kb_engine* e) {
+  if (rc != KB_OK) throw std::runtime_error(std::string(what) + ": " + kb_last_error(e) + " [" + kb_status_str(rc) + "]");
+}
+
+// One engine on device 0, single GPU
+struct Engine {
+  kb_engine* h = nullptr;
+  Engine() {
     kb_engine_opts eo{}; eo.abi_version = KB_ABI_VERSION; eo.device = 0; eo.rank = 0; eo.world_size = 1;
-    kb_engine* eng = nullptr;
-    int rc = kb_engine_create(&eo, &eng);
-    if (rc != KB_OK) throw std::runtime_error(std::string("kb_engine_create: ") + kb_last_error(nullptr) + " [" + kb_status_str(rc) + "]");
-    struct Guard { kb_engine* e; ~Guard() { kb_engine_destroy(e); } } guard{eng};
-    rc = kb_session_load(eng, &s, &conf);
-    if (rc != KB_OK) throw std::runtime_error(std::string("kb_session_load: ") + kb_last_error(eng) + " [" + kb_status_str(rc) + "]");
-    std::vector<kb_decision> dec(std::max(1u, f.T));
-    kb_stats st{};
-    rc = backfill ? kb_backfill(eng, dec.data(), &st) : kb_allocate(eng, dec.data(), &st);
-    if (rc != KB_OK) throw std::runtime_error(std::string(backfill ? "kb_backfill: " : "kb_allocate: ") + kb_last_error(eng) + " [" + kb_status_str(rc) + "]");
-    // replay in call order through the session's own Allocate / Pipeline (gang dispatch, Binder.Bind happen there)
-    std::vector<uint32_t> order;
-    for (uint32_t t = 0; t < f.T; ++t) if (dec[t].kind == KB_KIND_ALLOCATED || dec[t].kind == KB_KIND_PIPELINED) order.push_back(t);
-    std::sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return dec[a].step < dec[b].step; });
-    for (uint32_t t : order) {
-      if (dec[t].kind == KB_KIND_ALLOCATED) ssn->Allocate(f.tasks[t], f.nodeNames[dec[t].node]);
-      else ssn->Pipeline(f.tasks[t], f.nodeNames[dec[t].node]);
-    }
+    Check(kb_engine_create(&eo, &h), "kb_engine_create", nullptr);
+  }
+  ~Engine() { if (h) kb_engine_destroy(h); }
+  Engine(const Engine&) = delete;
+  Engine& operator=(const Engine&) = delete;
+};
+
+// One action on the GPU: flatten the session as it is NOW -> kb_session_load -> kb_allocate | kb_backfill -> replay the
+// decisions through the session's own Allocate / Pipeline.  Every action flattens afresh, so "allocate, backfill" (the
+// default list, pkg/scheduler/util.go:31-42) is two such calls, exactly like the reference runs two Execute()s on one
+// session.  (A shim that wants to save the second flatten + upload can call kb_allocate and kb_backfill back to back on
+// one loaded session instead: see INTEGRATION.md.)
+inline void ExecuteOnGpu(framework::Session* ssn, const bool backfill) {
+  PluginConf pc(*ssn);
+  Flat f = Flatten(*ssn);
+  kb_snapshot s = SnapshotOf(f);
+  Engine eng;
+  Check(kb_session_load(eng.h, &s, &pc.conf), "kb_session_load", eng.h);
+  std::vector<kb_decision> dec(std::max(1u, f.T));
+  kb_stats st{};
+  Check(backfill ? kb_backfill(eng.h, dec.data(), &st) : kb_allocate(eng.h, dec.data(), &st), backfill ? "kb_backfill" : "kb_allocate", eng.h);
+  // replay in call order through the session's own Allocate / Pipeline (gang dispatch, Binder.Bind happen there)
+  std::vector<uint32_t> order;
+  for (uint32_t t = 0; t < f.T; ++t) if (dec[t].kind == KB_KIND_ALLOCATED || dec[t].kind == KB_KIND_PIPELINED) order.push_back(t);
+  std::sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return dec[a].step < dec[b].step; });
+  for (uint32_t t : order) {
+    if (dec[t].kind == KB_KIND_ALLOCATED) ssn->Allocate(f.tasks[t], f.nodeNames[dec[t].node]);
+    else ssn->Pipeline(f.tasks[t], f.nodeNames[dec[t].node]);
   }
 }
 
@@ -593,5 +713,197 @@ class backfillAction : public framework::Action {
 };
 inline std::unique_ptr<framework::Action> New() { return std::make_unique<backfillAction>(); }
 }}  // namespace actions::backfill
+
+// ---------------------------------------------------------------------------------------------- actions/cycle
+// The configured action list ("reclaim, allocate, backfill, preempt", config/kube-batch-conf.yaml:1) as ONE kb_cycle on the
+// device, handed out to the action shells: the twin of go/kbgpu/cycle.go.  The first shell that runs in a session flattens
+// it as opened, loads it with its Running tasks and runs the whole list; every shell then replays only its own slice of the
+// result (`bounds`) through the session's own Evict / Pipeline / Allocate and framework::Statement.  A refusal of the engine
+// throws (no CPU fallback), in that shell and in every later shell of the same session.
+namespace actions { namespace cycle {
+
+// kb_running: the Running tasks of the session one by one (cycle.go::flattenRunning, builder.py meta["running"]).  No
+// inter-pod terms are flattened here, so no task is an affinity group member and aff_group_off / aff_group stay NULL.
+struct Running {
+  std::vector<std::shared_ptr<api::TaskInfo>> tasks;  // clones of the nodes' copies: what reclaim / preempt evict
+  std::vector<uint32_t> node, job, present, uid_rank, flags;
+  std::vector<double> resreq;                         // [R][n]
+  std::vector<int32_t> prio, waiting;                 // waiting: [J]
+  std::vector<int64_t> ctime;
+};
+
+inline Running FlattenRunning(const framework::Session& ssn, const allocate::Flat& f) {
+  std::map<std::string, uint32_t> jidx;
+  for (uint32_t j = 0; j < f.jobIDs.size(); ++j) jidx[f.jobIDs[j]] = j;
+  Running r;
+  std::vector<uint32_t> nodeOf;
+  for (uint32_t ni = 0; ni < f.nodeNames.size(); ++ni) {
+    for (auto& kv : ssn.Nodes.at(f.nodeNames[ni])->Tasks) {
+      auto& t = kv.second;
+      if (t->Status != api::Running) continue;        // reclaim.go:127, preempt.go:105
+      if (!jidx.count(t->Job)) continue;              // reclaim.go:131: tasks of unknown jobs are never candidates
+      r.tasks.push_back(t->Clone());                  // reclaim.go:135-136: a clone, so the node's copy keeps its status
+      nodeOf.push_back(ni);
+    }
+  }
+  const uint32_t n = (uint32_t)r.tasks.size(), n1 = std::max(1u, n);
+  std::vector<std::string> uids;
+  for (auto& t : r.tasks) uids.push_back(t->UID);
+  std::sort(uids.begin(), uids.end());
+  r.node.assign(n1, 0); r.job = r.present = r.uid_rank = r.flags = r.node;
+  r.resreq.assign((size_t)f.R * n1, 0); r.prio.assign(n1, 0); r.ctime.assign(n1, 0);
+  for (uint32_t i = 0; i < n; ++i) {
+    auto& t = *r.tasks[i];
+    r.node[i] = nodeOf[i];
+    r.job[i] = jidx.at(t.Job);
+    allocate::resourceVec(t.Resreq, f.dims, &r.resreq[i], n, &r.present[i]);
+    r.prio[i] = t.Priority;
+    r.uid_rank[i] = (uint32_t)(std::lower_bound(uids.begin(), uids.end(), t.UID) - uids.begin());
+    if (t.pod) {
+      r.ctime[i] = t.pod->CreationTimestamp;
+      const std::string& cn = t.pod->PriorityClassName;                    // conformance.go:45-53
+      if (cn == "system-cluster-critical" || cn == "system-node-critical" || t.Namespace == "kube-system") r.flags[i] |= KB_RUNNING_CRITICAL;
+    }
+  }
+  r.waiting.assign(std::max<size_t>(1, f.jobIDs.size()), 0);
+  for (uint32_t j = 0; j < f.jobIDs.size(); ++j) {     // WaitingTaskNum (job_info.go:396-405): 0 unless an earlier action pipelined tasks
+    auto& idx = ssn.Jobs.at(f.jobIDs[j])->TaskStatusIndex;
+    auto it = idx.find(api::Pipelined);
+    r.waiting[j] = it == idx.end() ? 0 : (int32_t)it->second.size();
+  }
+  return r;
+}
+
+class Cycle : public std::enable_shared_from_this<Cycle> {
+ public:
+  // `actions`: the configured list restricted to the four built-ins, in order.  A name may appear once: a shell finds its
+  // slice of the result by its name.
+  explicit Cycle(std::vector<std::string> actions) : actions_(std::move(actions)) {
+    for (size_t i = 0; i < actions_.size(); ++i) {
+      if (!actionID(actions_[i], nullptr)) throw std::runtime_error("kbgpu: unknown action \"" + actions_[i] + "\"");
+      for (size_t k = 0; k < i; ++k) if (actions_[k] == actions_[i]) throw std::runtime_error("kbgpu: action \"" + actions_[i] + "\" is listed twice");
+    }
+  }
+  // The four shells (framework::Action, actions/factory.go:28-33); they keep this Cycle alive
+  std::vector<std::unique_ptr<framework::Action>> Actions();
+
+  void Execute(framework::Session* ssn, const std::string& name) { ensure(ssn); replay(ssn, name); }
+
+ private:
+  static bool actionID(const std::string& name, uint8_t* id) {
+    static const std::map<std::string, uint8_t> ids = {{"reclaim", KB_ACT_RECLAIM}, {"allocate", KB_ACT_ALLOCATE}, {"backfill", KB_ACT_BACKFILL}, {"preempt", KB_ACT_PREEMPT}};
+    auto it = ids.find(name);
+    if (it == ids.end()) return false;
+    if (id) *id = it->second;
+    return true;
+  }
+  // the whole list once per session
+  void ensure(framework::Session* ssn) {
+    if (uid_ == ssn->UID) { if (!failed_.empty()) throw std::runtime_error(failed_); return; }
+    uid_ = ssn->UID;
+    failed_.clear();
+    try { run(ssn); } catch (const std::exception& e) { failed_ = e.what(); throw; }
+  }
+  void run(framework::Session* ssn) {
+    allocate::PluginConf pc(*ssn);
+    flat_ = allocate::Flatten(*ssn);
+    kb_snapshot s = allocate::SnapshotOf(flat_);
+    if (!engine_) engine_ = std::make_unique<allocate::Engine>();
+    kb_engine* e = engine_->h;
+    allocate::Check(kb_session_load(e, &s, &pc.conf), "kb_session_load", e);
+    running_ = FlattenRunning(*ssn, flat_);
+    Running& rf = running_;
+    const uint32_t n = (uint32_t)rf.tasks.size();
+    kb_running run{};
+    run.n = n;
+    run.node = rf.node.data(); run.job = rf.job.data(); run.resreq = rf.resreq.data(); run.res_present = rf.present.data();
+    run.prio = rf.prio.data(); run.ctime = rf.ctime.data(); run.uid_rank = rf.uid_rank.data(); run.flags = rf.flags.data();
+    run.job_waiting0 = rf.waiting.data();
+    allocate::Check(kb_session_load_running(e, &s, &run), "kb_session_load_running", e);
+    std::vector<uint8_t> acts(actions_.size());
+    for (size_t i = 0; i < actions_.size(); ++i) actionID(actions_[i], &acts[i]);
+    dec_.assign(std::max(1u, flat_.T), kb_decision{});
+    std::vector<uint8_t> ev(std::max(1u, n), 0);
+    order_.assign(std::max(1u, n), 0);
+    bounds_.assign(2 * std::max<size_t>(1, acts.size()), 0);
+    kb_stats st{};
+    allocate::Check(kb_cycle(e, acts.data(), (uint32_t)acts.size(), dec_.data(), ev.data(), order_.data(), bounds_.data(), &st), "kb_cycle", e);
+    dec_.resize(flat_.T);
+    order_.resize(n);
+    evicted_.assign(n, false);
+    for (uint32_t i = 0; i < n; ++i) evicted_[i] = ev[i] != 0;
+  }
+  // the decisions action `name` made, in the order the reference would have made the calls (cycle.go::replay)
+  void replay(framework::Session* ssn, const std::string& name) {
+    size_t idx = 0;
+    while (idx < actions_.size() && actions_[idx] != name) ++idx;
+    if (idx == actions_.size()) throw std::runtime_error("kbgpu: action \"" + name + "\" is not part of the configured cycle");
+    const uint32_t lo_step = idx ? bounds_[2 * idx - 2] : 0, lo_ev = idx ? bounds_[2 * idx - 1] : 0;
+    const uint32_t hi_step = bounds_[2 * idx], hi_ev = bounds_[2 * idx + 1];
+    // evictions of this action, in cache.Evict order
+    std::vector<uint32_t> evs;
+    for (uint32_t i = 0; i < evicted_.size(); ++i) if (evicted_[i] && order_[i] >= lo_ev && order_[i] < hi_ev) evs.push_back(i);
+    std::sort(evs.begin(), evs.end(), [&](uint32_t a, uint32_t b) { return order_[a] < order_[b]; });
+    // placements of this action, in step order
+    std::vector<uint32_t> pls;
+    for (uint32_t t = 0; t < dec_.size(); ++t) {
+      const kb_decision& d = dec_[t];
+      if ((d.kind == KB_KIND_ALLOCATED || d.kind == KB_KIND_PIPELINED) && d.step != 0xFFFFFFFFu && d.step >= lo_step && d.step < hi_step) pls.push_back(t);
+    }
+    std::sort(pls.begin(), pls.end(), [&](uint32_t a, uint32_t b) { return dec_[a].step < dec_[b].step; });
+    auto nodeOf = [&](uint32_t t) { return flat_.nodeNames.at((size_t)dec_[t].node); };
+    if (name == "preempt") {
+      // the engine only reports committed statements (preempt.go:121-131); one Statement replays them: evictions first, so
+      // that node.Releasing covers the pipelined tasks (node_info.go:190-192), then Commit sends the evictions to the cache
+      framework::Statement stmt(ssn);
+      for (uint32_t i : evs) stmt.Evict(running_.tasks[i], "preempt");
+      for (uint32_t t : pls) stmt.Pipeline(flat_.tasks[t], nodeOf(t));
+      stmt.Commit();
+    } else if (name == "reclaim") {
+      // reclaim.go:157-185 interleaves: the victims of one reclaimer, then its Pipeline.  Replaying all evictions of the
+      // action first and the pipelines after them leaves the same session state (evictions only add to Releasing).
+      for (uint32_t i : evs) ssn->Evict(running_.tasks[i], "reclaim");
+      for (uint32_t t : pls) ssn->Pipeline(flat_.tasks[t], nodeOf(t));
+    } else {                                           // allocate, backfill
+      for (uint32_t t : pls) {
+        if (dec_[t].kind == KB_KIND_ALLOCATED) ssn->Allocate(flat_.tasks[t], nodeOf(t));   // dispatches when ssn.JobReady (session.go:277-285)
+        else ssn->Pipeline(flat_.tasks[t], nodeOf(t));
+      }
+      // backfill's phantom tasks (Allocated on no node, step none: session.go:241-262) are not replayed: the reference itself
+      // calls that state "will be corrected in next scheduling loop"
+    }
+  }
+
+  std::vector<std::string> actions_;
+  std::unique_ptr<allocate::Engine> engine_;
+  std::string uid_, failed_;                           // the session the cached result belongs to; its refusal, if any
+  allocate::Flat flat_;
+  Running running_;
+  std::vector<kb_decision> dec_;
+  std::vector<bool> evicted_;
+  std::vector<uint32_t> order_, bounds_;
+};
+
+// The drop-in shell of one of the four actions: same Name(), same framework::Action interface (framework/interface.go:20-32)
+class action : public framework::Action {
+ public:
+  action(std::string name, std::shared_ptr<Cycle> cycle) : name_(std::move(name)), cycle_(std::move(cycle)) {}
+  std::string Name() const override { return name_; }
+  void Execute(framework::Session* ssn) override { cycle_->Execute(ssn, name_); }
+ private:
+  std::string name_;
+  std::shared_ptr<Cycle> cycle_;
+};
+
+inline std::vector<std::unique_ptr<framework::Action>> Cycle::Actions() {
+  std::vector<std::unique_ptr<framework::Action>> out;
+  for (const char* name : {"reclaim", "allocate", "backfill", "preempt"}) out.push_back(std::make_unique<action>(name, shared_from_this()));
+  return out;
+}
+
+// New(actions)->Actions(): a Cycle is shared by its shells
+inline std::shared_ptr<Cycle> New(const std::vector<std::string>& actions) { return std::make_shared<Cycle>(actions); }
+
+}}  // namespace actions::cycle
 
 }  // namespace kb
