@@ -173,11 +173,17 @@ func (c *Cycle) run(ssn *framework.Session) error {
 	run.resreq, run.prio, run.ctime = a.f64(rf.resreq), a.i32(rf.prio), a.i64(rf.ctime)
 	run.uid_rank, run.flags, run.job_waiting0 = a.u32(rf.uidRank), a.u32(rf.flags), a.i32(rf.waiting)
 	run.aff_group_off, run.aff_group = a.u32(rf.affGroupOff), a.u32(append(rf.affGroup, 0)) // a.u32 needs one element
-	if rc := C.kb_session_load_running(c.engine.h, snap, run); rc != 0 {
-		if rc == C.KB_E_UNSUPPORTED_FEATURE {
-			return &ErrUnsupported{C.GoString(C.kb_last_error(c.engine.h))}
+	evicts := false // only reclaim and preempt read the Running tasks: without them a session the victim walk cannot run is not refused
+	for _, name := range c.actions {
+		evicts = evicts || name == "reclaim" || name == "preempt"
+	}
+	if evicts {
+		if rc := C.kb_session_load_running(c.engine.h, snap, run); rc != 0 {
+			if rc == C.KB_E_UNSUPPORTED_FEATURE {
+				return &ErrUnsupported{C.GoString(C.kb_last_error(c.engine.h))}
+			}
+			return c.engine.err("kb_session_load_running", rc)
 		}
-		return c.engine.err("kb_session_load_running", rc)
 	}
 	acts := make([]C.uint8_t, len(c.actions))
 	for i, name := range c.actions {

@@ -117,7 +117,8 @@ func (a *atomTable) of(req v1.NodeSelectorRequirement, field bool) uint32 {
 }
 
 // never is an atom no node satisfies: a required term without expressions matches nothing
-// (v1helper.MatchNodeSelectorTerms skips it), so a pod whose every term is empty fits nowhere.
+// (v1helper.MatchNodeSelectorTerms skips it), so a pod whose every term is empty fits nowhere; a preferred term without
+// expressions adds its weight nowhere.
 func (a *atomTable) never() uint32 {
 	return a.of(v1.NodeSelectorRequirement{Key: "\x00never", Operator: v1.NodeSelectorOpIn, Values: []string{"\x00"}}, false)
 }
@@ -370,6 +371,9 @@ func Flatten(ssn *framework.Session) (*Flat, error) {
 			var as []uint32
 			for _, e := range p.Preference.MatchExpressions { // MatchFields are ignored by the priority (node_affinity.go:52-56)
 				as = append(as, atoms.of(e, false))
+			}
+			if len(as) == 0 { // NodeSelectorRequirementsAsSelector(nil) is labels.Nothing() (helpers.go:205-208): the term matches no node
+				as = []uint32{atoms.never()}
 			}
 			terms[ti].pref = append(terms[ti].pref, as)
 			terms[ti].prefW = append(terms[ti].prefW, p.Weight)

@@ -18,7 +18,9 @@
 #pragma once
 
 #include <algorithm>
+#include <cerrno>
 #include <cmath>
+#include <cstdlib>
 #include <cstdint>
 #include <functional>
 #include <map>
@@ -26,6 +28,7 @@
 #include <set>
 #include <stdexcept>
 #include <string>
+#include <tuple>
 #include <vector>
 
 #include "../../include/kbgpu.h"
@@ -75,8 +78,35 @@ enum TaskStatus { Pending = 1, Allocated = 2, Pipelined = 4, Binding = 8, Bound 
                   Succeeded = 128, Failed = 256, Unknown = 512 };                     // api/types.go:20-54
 inline bool AllocatedStatus(int s) { return s == Bound || s == Binding || s == Running || s == Allocated; }   // api/helpers.go:64-71
 
+// v1.Affinity (k8s.io/api/core/v1/types.go).  A nil pointer is the Go nil; an empty list is an empty list.
+struct NodeSelectorRequirement { std::string Key, Operator; std::vector<std::string> Values; };   // In NotIn Exists DoesNotExist Gt Lt
+struct NodeSelectorTerm { std::vector<NodeSelectorRequirement> MatchExpressions, MatchFields; };
+struct NodeSelector { std::vector<NodeSelectorTerm> NodeSelectorTerms; };
+struct PreferredSchedulingTerm { int32_t Weight = 0; NodeSelectorTerm Preference; };
+struct NodeAffinity {
+  std::shared_ptr<NodeSelector> RequiredDuringSchedulingIgnoredDuringExecution;
+  std::vector<PreferredSchedulingTerm> PreferredDuringSchedulingIgnoredDuringExecution;
+};
+struct LabelSelectorRequirement { std::string Key, Operator; std::vector<std::string> Values; };  // In NotIn Exists DoesNotExist
+struct LabelSelector { std::map<std::string, std::string> MatchLabels; std::vector<LabelSelectorRequirement> MatchExpressions; };
+struct PodAffinityTerm {
+  std::shared_ptr<api::LabelSelector> LabelSelector;  // nil: labels.Nothing() (LabelSelectorAsSelector)
+  std::vector<std::string> Namespaces;                // empty: the owning pod's namespace
+  std::string TopologyKey;
+};
+struct WeightedPodAffinityTerm { int32_t Weight = 0; api::PodAffinityTerm PodAffinityTerm; };
+struct PodAffinity {                                  // also v1.PodAntiAffinity
+  std::vector<api::PodAffinityTerm> RequiredDuringSchedulingIgnoredDuringExecution;
+  std::vector<WeightedPodAffinityTerm> PreferredDuringSchedulingIgnoredDuringExecution;
+};
+struct Affinity {
+  std::shared_ptr<api::NodeAffinity> NodeAffinity;
+  std::shared_ptr<api::PodAffinity> PodAffinity, PodAntiAffinity;
+};
+
 struct Pod {                                          // the v1.Pod fields the path reads (util/test_utils.go:66-93 BuildPod)
   std::string Namespace, Name, UID, NodeName, Phase = "Pending", GroupName;
+  std::shared_ptr<api::Affinity> Affinity;            // Spec.Affinity
   ResourceList Requests;                              // one container
   std::vector<ResourceList> InitRequests;
   std::map<std::string, std::string> Labels, NodeSelector;
@@ -482,6 +512,23 @@ struct Flat {
   std::vector<int64_t> node_alloc_cpu, node_alloc_mem, node_nz_cpu, node_nz_mem, task_nz_cpu, task_nz_mem, task_ctime, job_ctime, queue_ctime;
   std::vector<int32_t> node_pods, node_max_pods, task_prio, job_min_avail, job_ready0, job_prio, queue_weight;
   std::vector<uint64_t> node_labels, node_taints, node_ports, task_sel_req, task_aff, task_tol, task_port_own, task_port_conflict;
+  std::vector<uint32_t> task_n_pref;                  // [T]
+  std::vector<uint64_t> task_pref;                    // [KB_MAX_PREF_TERMS][W][T]
+  std::vector<int32_t> task_pref_w;                   // [KB_MAX_PREF_TERMS][T]
+  uint32_t snap_flags = 0;                            // KB_SNAPSHOT_*
+  // kb_pod_affinity (FlattenPodAffinity); `on` is false when no pod of the session carries inter-pod terms
+  struct PodAff {
+    bool on = false;
+    uint32_t n_keysets = 0, n_groups = 0, n_kinds = 0;
+    int32_t first_unbound = -1;
+    std::vector<int32_t> node_domain, group_count0, group_total0, task_need, task_kind, node_kind_count0, weight_kind, weight_keyset;
+    std::vector<uint32_t> keyset_domains, group_keyset, task_weight_off, task_xgroup_off, task_xgroup;   // xgroup: empty when <= 64 groups
+    std::vector<uint64_t> task_forbid, task_contrib;
+    std::vector<uint8_t> kind_unbound;
+    std::vector<int64_t> weight_value;
+    std::map<const api::Pod*, std::vector<uint32_t>> member_groups;   // listed pods that are members: their groups, ascending
+    kb_pod_affinity c{};                              // filled by SnapshotOf over the vectors above
+  } pa;
 };
 
 inline void resourceVec(const api::Resource& r, const std::vector<std::string>& dims, double* out, size_t stride, uint32_t* present) {
@@ -490,6 +537,71 @@ inline void resourceVec(const api::Resource& r, const std::vector<std::string>& 
   for (auto& kv : r.ScalarResources) { size_t k = std::find(dims.begin(), dims.end(), kv.first) - dims.begin(); out[k * stride] = kv.second; p |= 1u << k; }
   if (present) *present = p;
 }
+
+// "kbgpu: unsupported session: ..." — what the Go shim returns as *ErrUnsupported
+inline std::runtime_error Unsupported(const std::string& why) { return std::runtime_error("kbgpu: unsupported session: " + why); }
+
+// strconv.ParseInt(s, 10, 64)
+inline bool parseInt64(const std::string& s, int64_t* out) {
+  size_t i = (!s.empty() && (s[0] == '+' || s[0] == '-')) ? 1 : 0;
+  if (i == s.size()) return false;
+  for (size_t k = i; k < s.size(); ++k) if (s[k] < '0' || s[k] > '9') return false;
+  errno = 0;
+  char* end = nullptr;
+  long long v = std::strtoll(s.c_str(), &end, 10);
+  if (errno == ERANGE) return false;
+  *out = v;
+  return true;
+}
+
+// labels.Requirement.Matches of a requirement labels.NewRequirement accepts; a requirement it refuses matches nothing (the vendored
+// callers treat the error as "no match": MatchNodeSelectorTerms, NodeSelectorRequirementsAsSelector)
+inline bool labelRequirementHolds(const std::map<std::string, std::string>& labels, const std::string& key, const std::string& op,
+                                  const std::vector<std::string>& values) {
+  auto it = labels.find(key);
+  const bool has = it != labels.end();
+  auto in = [&] { return has && std::find(values.begin(), values.end(), it->second) != values.end(); };
+  if (op == "In") return !values.empty() && in();
+  if (op == "NotIn") return !values.empty() && !in();
+  if (op == "Exists") return values.empty() && has;
+  if (op == "DoesNotExist") return values.empty() && !has;
+  if (op == "Gt" || op == "Lt") {                     // one integer value; a label that does not parse fails the match
+    int64_t rv, lv;
+    if (values.size() != 1 || !parseInt64(values[0], &rv) || !has || !parseInt64(it->second, &lv)) return false;
+    return op == "Gt" ? lv > rv : lv < rv;
+  }
+  return false;
+}
+
+// One node-selector requirement evaluated ONCE per node (flatten.go reqAtom / atomTable): a nodeSelector pair (as In), a required or
+// preferred node-affinity MatchExpression, or a MatchFields requirement.  Identical requirements written identically share the atom.
+struct AtomTable {
+  struct Req { bool field; std::string key, op; std::vector<std::string> values; };
+  std::map<std::tuple<bool, std::string, std::string, std::vector<std::string>>, uint32_t> ids;
+  std::vector<Req> reqs;
+  uint32_t of(const api::NodeSelectorRequirement& r, bool field) {
+    auto k = std::make_tuple(field, r.Key, r.Operator, r.Values);
+    auto it = ids.find(k);
+    if (it != ids.end()) return it->second;
+    uint32_t id = (uint32_t)reqs.size();
+    ids.emplace(k, id);
+    reqs.push_back({field, r.Key, r.Operator, r.Values});
+    return id;
+  }
+  // an atom no node satisfies: a required term without expressions, or a preferred term without expressions
+  // (NodeSelectorRequirementsAsSelector of an empty list is labels.Nothing(), helpers.go:205-208)
+  uint32_t never() { return of({"\x01never", "In", {"\x01"}}, false); }
+  bool holds(uint32_t a, const api::Node& node) const {
+    const Req& r = reqs[a];
+    if (!r.field) return labelRequirementHolds(node.Labels, r.key, r.op, r.values);
+    // NodeSelectorRequirementsAsFieldSelector (helpers.go:239-267): In / NotIn with one value, against fields.Set{"metadata.name": ...}
+    if ((r.op != "In" && r.op != "NotIn") || r.values.size() != 1) return false;
+    const std::string v = r.key == "metadata.name" ? node.Name : std::string();
+    return r.op == "In" ? v == r.values[0] : v != r.values[0];
+  }
+};
+
+inline void FlattenPodAffinity(const framework::Session& ssn, Flat& f);
 
 // What the Go shim's Flatten(ssn) does (INTEGRATION.md §"What Flatten must compute"); mirrors builder.py::flatten.
 inline Flat Flatten(const framework::Session& ssn) {
@@ -516,17 +628,48 @@ inline Flat Flatten(const framework::Session& ssn) {
   }
   f.T = (uint32_t)f.tasks.size();
   std::sort(uids.begin(), uids.end());
-  // atoms: selector requirements (nodeSelector pairs), NoSchedule/NoExecute taints, host ports
-  std::map<std::pair<std::string, std::string>, uint32_t> labelAtoms;
+  // atoms: selector requirements, NoSchedule/NoExecute taints, host ports.  Per task in task order: the nodeSelector pairs (as In,
+  // ascending key), the required node-affinity terms, the preferred ones (flatten.go, builder.py::flatten)
+  AtomTable atoms;
+  struct TaskTerms { std::vector<uint32_t> sel; std::vector<std::vector<uint32_t>> aff, pref; std::vector<int32_t> prefW; };
+  std::vector<TaskTerms> terms(f.T);
+  for (uint32_t t = 0; t < f.T; ++t) {
+    const api::TaskInfo& ti = *f.tasks[t];
+    const api::Pod& p = *ti.pod;
+    for (auto& kv : p.NodeSelector) terms[t].sel.push_back(atoms.of({kv.first, "In", {kv.second}}, false));   // labels.SelectorFromSet
+    if (!p.Affinity || !p.Affinity->NodeAffinity) continue;
+    const api::NodeAffinity& na = *p.Affinity->NodeAffinity;
+    if (na.RequiredDuringSchedulingIgnoredDuringExecution) {                      // predicates.go:944-968
+      for (auto& term : na.RequiredDuringSchedulingIgnoredDuringExecution->NodeSelectorTerms) {
+        if (term.MatchExpressions.empty() && term.MatchFields.empty()) continue;   // matches nothing (MatchNodeSelectorTerms)
+        std::vector<uint32_t> as;
+        for (auto& e : term.MatchExpressions) as.push_back(atoms.of(e, false));
+        for (auto& e : term.MatchFields) as.push_back(atoms.of(e, true));
+        terms[t].aff.push_back(as);
+      }
+      if (terms[t].aff.empty()) terms[t].aff.push_back({atoms.never()});
+      if (terms[t].aff.size() > KB_MAX_AFF_TERMS)
+        throw Unsupported("pod " + ti.Namespace + "/" + ti.Name + " has " + std::to_string(terms[t].aff.size()) + " required node-affinity terms > KB_MAX_AFF_TERMS");
+    }
+    for (auto& pt : na.PreferredDuringSchedulingIgnoredDuringExecution) {         // node_affinity.go:34-77
+      if (pt.Weight == 0) continue;
+      std::vector<uint32_t> as;
+      for (auto& e : pt.Preference.MatchExpressions) as.push_back(atoms.of(e, false));   // MatchFields are ignored by the priority
+      if (as.empty()) as.push_back(atoms.never());
+      terms[t].pref.push_back(as);
+      terms[t].prefW.push_back(pt.Weight);
+    }
+    if (terms[t].pref.size() > KB_MAX_PREF_TERMS)
+      throw Unsupported("pod " + ti.Namespace + "/" + ti.Name + " has " + std::to_string(terms[t].pref.size()) + " preferred node-affinity terms > KB_MAX_PREF_TERMS");
+  }
   std::map<std::tuple<std::string, std::string, std::string>, uint32_t> taintAtoms;
   std::map<std::tuple<std::string, std::string, int>, uint32_t> portAtoms;
   auto san = [](const api::Pod::HostPort& h) { return std::make_tuple(h.HostIP.empty() ? std::string("0.0.0.0") : h.HostIP, h.Protocol.empty() ? std::string("TCP") : h.Protocol, h.Port); };
-  for (auto& t : f.tasks) for (auto& kv : t->pod->NodeSelector) labelAtoms.emplace(std::make_pair(kv.first, kv.second), (uint32_t)labelAtoms.size());
   for (auto& n : nodes) for (auto& t : n->node->Taints) if (t.Effect == "NoSchedule" || t.Effect == "NoExecute") taintAtoms.emplace(std::make_tuple(t.Key, t.Value, t.Effect), (uint32_t)taintAtoms.size());
   for (auto& jk : ssn.Jobs) for (auto& tk : jk.second->Tasks) for (auto& h : tk.second->pod->HostPorts) if (h.Port > 0) portAtoms.emplace(san(h), (uint32_t)portAtoms.size());
-  size_t need = std::max({labelAtoms.size(), taintAtoms.size(), portAtoms.size(), (size_t)1});
+  size_t need = std::max({atoms.reqs.size(), taintAtoms.size(), portAtoms.size(), (size_t)1});
   f.W = (uint32_t)((need + 63) / 64);
-  if (f.W > KB_MAX_W) throw std::runtime_error("too many atoms for KB_MAX_W");
+  if (f.W > KB_MAX_W) throw Unsupported(std::to_string(need) + " label / taint / port atoms > 64 x KB_MAX_W");
   const uint32_t R = f.R, W = f.W, N = f.N, T = f.T, J = f.J, Q = f.Q;
   auto setbit = [](std::vector<uint64_t>& a, size_t stride, size_t i, uint32_t atom) { a[(atom / 64) * stride + i] |= 1ull << (atom % 64); };
   // nodes
@@ -555,7 +698,7 @@ inline Flat Flatten(const framework::Session& ssn) {
       f.node_nz_mem[i] += p.Requests.count("memory") ? (int64_t)p.Requests.at("memory") : 200ll * 1024 * 1024;             // non_zero.go:38
       for (auto& h : p.HostPorts) if (h.Port > 0) setbit(f.node_ports, N, i, portAtoms.at(san(h)));
     }
-    for (auto& la : labelAtoms) { auto it = n.node->Labels.find(la.first.first); if (it != n.node->Labels.end() && it->second == la.first.second) setbit(f.node_labels, N, i, la.second); }
+    for (uint32_t a = 0; a < atoms.reqs.size(); ++a) if (atoms.holds(a, *n.node)) setbit(f.node_labels, N, i, a);
     for (auto& t : n.node->Taints) { auto it = taintAtoms.find(std::make_tuple(t.Key, t.Value, t.Effect)); if (it != taintAtoms.end()) setbit(f.node_taints, N, i, it->second); }
   }
   // tasks
@@ -564,12 +707,22 @@ inline Flat Flatten(const framework::Session& ssn) {
   f.task_nz_cpu.assign(std::max(1u, T), 0); f.task_nz_mem = f.task_ctime = f.task_nz_cpu; f.task_prio.assign(std::max(1u, T), 0);
   f.task_sel_req.assign((size_t)W * std::max(1u, T), 0); f.task_tol = f.task_port_own = f.task_port_conflict = f.task_sel_req;
   f.task_aff.assign((size_t)KB_MAX_AFF_TERMS * W * std::max(1u, T), 0);
+  f.task_n_pref.assign(std::max(1u, T), 0); f.task_pref.assign((size_t)KB_MAX_PREF_TERMS * W * std::max(1u, T), 0);
+  f.task_pref_w.assign((size_t)KB_MAX_PREF_TERMS * std::max(1u, T), 0);
   for (uint32_t t = 0; t < T; ++t) {
     auto& ti = *f.tasks[t]; auto& p = *ti.pod;
     resourceVec(ti.Resreq, f.dims, &f.task_resreq[t], T, &f.task_res_present[t]); resourceVec(ti.InitResreq, f.dims, &f.task_initreq[t], T, nullptr);
     f.task_nz_cpu[t] = p.Requests.count("cpu") ? (int64_t)std::ceil(p.Requests.at("cpu") * 1000.0 - 1e-9) : 100;
     f.task_nz_mem[t] = p.Requests.count("memory") ? (int64_t)p.Requests.at("memory") : 200ll * 1024 * 1024;
-    for (auto& kv : p.NodeSelector) setbit(f.task_sel_req, T, t, labelAtoms.at({kv.first, kv.second}));
+    for (uint32_t a : terms[t].sel) setbit(f.task_sel_req, T, t, a);
+    f.task_n_aff[t] = (uint32_t)terms[t].aff.size();
+    for (size_t k = 0; k < terms[t].aff.size(); ++k) for (uint32_t a : terms[t].aff[k]) f.task_aff[(k * W + a / 64) * T + t] |= 1ull << (a % 64);
+    f.task_n_pref[t] = (uint32_t)terms[t].pref.size();
+    for (size_t k = 0; k < terms[t].pref.size(); ++k) {
+      f.task_pref_w[k * T + t] = terms[t].prefW[k];
+      for (uint32_t a : terms[t].pref[k]) f.task_pref[(k * W + a / 64) * T + t] |= 1ull << (a % 64);
+    }
+    if (!terms[t].pref.empty()) f.task_flags[t] |= KB_TASK_HAS_PREFERRED_NODE_AFFINITY;
     for (auto& ta : taintAtoms) for (auto& tol : p.Tolerations) {                // Toleration.ToleratesTaint, toleration.go:37-56
       if (!tol.Effect.empty() && tol.Effect != std::get<2>(ta.first)) continue;
       if (!tol.Key.empty() && tol.Key != std::get<0>(ta.first)) continue;
@@ -596,7 +749,326 @@ inline Flat Flatten(const framework::Session& ssn) {
   }
   f.queue_weight.assign(std::max(1u, Q), 0); f.queue_ctime.assign(std::max(1u, Q), 0);
   for (uint32_t q = 0; q < Q; ++q) { f.queue_weight[q] = queues[q]->Weight; f.queue_ctime[q] = queues[q]->CreationTimestamp; }
+  FlattenPodAffinity(ssn, f);
   return f;
+}
+
+// ---- inter-pod (anti)affinity: the twin of go/kbgpu/podaffinity.go::flattenPodAffinity (builder.py::flatten_pod_affinity) ----
+
+// What a term selects: GetNamespacesFromPodAffinityTerm + LabelSelectorAsSelector (topologies.go:25-49), with a canonical key:
+// the namespaces, then the requirements ascending (a MatchLabels pair is the requirement key In (value))
+struct TermProps {
+  std::set<std::string> ns;
+  bool nothing = false;                               // nil selector: labels.Nothing()
+  std::vector<std::tuple<std::string, std::string, std::vector<std::string>>> reqs;   // (key, op, values ascending)
+  std::string key;
+  bool matches(const api::Pod& pod) const {           // PodMatchesTermsNamespaceAndSelector (topologies.go:38-49)
+    if (!ns.count(pod.Namespace) || nothing) return false;
+    for (auto& r : reqs) if (!labelRequirementHolds(pod.Labels, std::get<0>(r), std::get<1>(r), std::get<2>(r))) return false;
+    return true;
+  }
+};
+
+inline TermProps propsOf(const api::Pod& owner, const api::PodAffinityTerm& term) {
+  TermProps p;
+  for (auto& n : term.Namespaces) p.ns.insert(n);
+  if (p.ns.empty()) p.ns.insert(owner.Namespace);
+  for (auto& n : p.ns) p.key += n + ",";
+  if (!term.LabelSelector) { p.nothing = true; p.key += "|nil"; return p; }
+  for (auto& kv : term.LabelSelector->MatchLabels) p.reqs.emplace_back(kv.first, "In", std::vector<std::string>{kv.second});
+  for (auto& e : term.LabelSelector->MatchExpressions) {     // labels.NewRequirement refuses what LabelSelectorAsSelector then returns
+    const bool valued = e.Operator == "In" || e.Operator == "NotIn";
+    if (!valued && e.Operator != "Exists" && e.Operator != "DoesNotExist")
+      throw Unsupported("invalid label selector in a pod (anti)affinity term: \"" + e.Operator + "\" is not a valid pod selector operator");
+    if (valued == e.Values.empty())
+      throw Unsupported("invalid label selector in a pod (anti)affinity term: operator " + e.Operator + (valued ? " needs values" : " takes no values"));
+    std::vector<std::string> v(e.Values);
+    std::sort(v.begin(), v.end());
+    v.erase(std::unique(v.begin(), v.end()), v.end());
+    p.reqs.emplace_back(e.Key, e.Operator, v);
+  }
+  std::sort(p.reqs.begin(), p.reqs.end());
+  p.key += "|sel";
+  for (auto& r : p.reqs) {
+    p.key += "|" + std::get<0>(r) + " " + std::get<1>(r);
+    for (auto& v : std::get<2>(r)) p.key += " " + v;
+  }
+  return p;
+}
+
+inline const std::vector<api::PodAffinityTerm>& requiredTerms(const api::Pod& pod, bool anti) {
+  static const std::vector<api::PodAffinityTerm> none;
+  if (!pod.Affinity) return none;
+  const auto& a = anti ? pod.Affinity->PodAntiAffinity : pod.Affinity->PodAffinity;
+  return a ? a->RequiredDuringSchedulingIgnoredDuringExecution : none;
+}
+inline const std::vector<api::WeightedPodAffinityTerm>& preferredTerms(const api::Pod& pod, bool anti) {
+  static const std::vector<api::WeightedPodAffinityTerm> none;
+  if (!pod.Affinity) return none;
+  const auto& a = anti ? pod.Affinity->PodAntiAffinity : pod.Affinity->PodAffinity;
+  return a ? a->PreferredDuringSchedulingIgnoredDuringExecution : none;
+}
+inline bool hasPodAffinity(const api::Pod& pod) { return pod.Affinity && (pod.Affinity->PodAffinity || pod.Affinity->PodAntiAffinity); }
+
+// pods with the same namespace, labels and (anti)affinity spec are interchangeable for every match below
+inline std::string podType(const api::Pod& pod) {
+  std::string s = pod.Namespace + '\x01';
+  for (auto& kv : pod.Labels) s += kv.first + "=" + kv.second + ",";
+  auto term = [&](const api::PodAffinityTerm& t) {
+    s += "{" + t.TopologyKey + "|";
+    for (auto& n : t.Namespaces) s += n + ",";
+    if (!t.LabelSelector) { s += "|nil}"; return; }
+    s += "|";
+    for (auto& kv : t.LabelSelector->MatchLabels) s += kv.first + "=" + kv.second + ",";
+    for (auto& e : t.LabelSelector->MatchExpressions) { s += e.Key + " " + e.Operator; for (auto& v : e.Values) s += " " + v; s += ","; }
+    s += "}";
+  };
+  for (const auto* a : {pod.Affinity ? pod.Affinity->PodAffinity.get() : nullptr, pod.Affinity ? pod.Affinity->PodAntiAffinity.get() : nullptr}) {
+    s += '\x01';
+    if (!a) { s += "nil"; continue; }
+    for (auto& t : a->RequiredDuringSchedulingIgnoredDuringExecution) term(t);
+    s += "/";
+    for (auto& w : a->PreferredDuringSchedulingIgnoredDuringExecution) { s += std::to_string(w.Weight); term(w.PodAffinityTerm); }
+  }
+  return s;
+}
+
+// Fills f.pa (f.pa.on stays false when no pod carries inter-pod terms), KB_TASK_HAS_POD_AFFINITY / KB_TASK_AFF_SELF_MATCH and
+// KB_SNAPSHOT_PLACED_POD_AFFINITY / KB_SNAPSHOT_LISTED_POD_WITHOUT_NODE.  Throws Unsupported where flattenPodAffinity returns
+// *ErrUnsupported.
+inline void FlattenPodAffinity(const framework::Session& ssn, Flat& f) {
+  const uint32_t N = f.N, T = f.T;
+  std::map<std::string, uint32_t> nidx;
+  for (uint32_t i = 0; i < N; ++i) nidx[f.nodeNames[i]] = i;
+  struct Placed { const api::Pod* pod; uint32_t node; bool unbound; };
+  // util.PodLister (plugins/util/util.go:37-85): AllocatedStatus tasks of the session's jobs, located by TaskInfo.NodeName
+  std::vector<Placed> listed;
+  bool any = false;
+  for (auto& id : f.jobIDs) {
+    for (auto& st : ssn.Jobs.at(id)->TaskStatusIndex) {
+      if (!api::AllocatedStatus(st.first)) continue;
+      for (auto& kv : st.second) {
+        const api::TaskInfo& t = *kv.second;
+        auto n = nidx.find(t.NodeName);
+        if (n == nidx.end()) { f.snap_flags |= KB_SNAPSHOT_LISTED_POD_WITHOUT_NODE; continue; }   // GetNodeInfo fails (kbgpu.h)
+        listed.push_back({t.pod.get(), n->second, t.pod->NodeName.empty()});
+        if (hasPodAffinity(*t.pod)) { any = true; f.snap_flags |= KB_SNAPSHOT_PLACED_POD_AFFINITY; }
+      }
+    }
+  }
+  // NodeInfo.Tasks of every node, whatever the status: what nodeInfo.Pods() hands the priority
+  std::vector<Placed> inTasks;
+  int32_t firstUnbound = -1;
+  for (uint32_t n = 0; n < N; ++n) {
+    for (auto& kv : ssn.Nodes.at(f.nodeNames[n])->Tasks) {
+      const api::Pod* pod = kv.second->pod.get();
+      const bool unbound = pod->NodeName.empty();
+      inTasks.push_back({pod, n, unbound});
+      if (unbound && firstUnbound < 0) firstUnbound = (int32_t)n;
+      if (hasPodAffinity(*pod)) { any = true; f.snap_flags |= KB_SNAPSHOT_PLACED_POD_AFFINITY; }
+    }
+  }
+  for (auto& t : f.tasks) if (hasPodAffinity(*t->pod)) any = true;
+  if (!any) return;
+  Flat::PodAff& pa = f.pa;
+  pa.on = true;
+  pa.first_unbound = firstUnbound;
+
+  // ---- pod types ----
+  std::map<std::string, int> typeID;
+  std::vector<const api::Pod*> reps;
+  auto typeOf = [&](const api::Pod* pod) {
+    auto ins = typeID.emplace(podType(*pod), (int)reps.size());
+    if (ins.second) reps.push_back(pod);
+    return ins.first->second;
+  };
+  std::vector<int> ptype(T), ltype, ttype;
+  std::set<int> pendSet;
+  for (uint32_t t = 0; t < T; ++t) { ptype[t] = typeOf(f.tasks[t]->pod.get()); pendSet.insert(ptype[t]); }
+  for (auto& p : listed) ltype.push_back(typeOf(p.pod));
+  for (auto& p : inTasks) ttype.push_back(typeOf(p.pod));
+  const std::vector<int> pendTypes(pendSet.begin(), pendSet.end());
+
+  // ---- key sets and domains ----
+  std::map<std::vector<std::string>, uint32_t> keysetID;
+  auto keysetOf = [&](std::vector<std::string> keys) -> uint32_t {
+    std::sort(keys.begin(), keys.end());
+    keys.erase(std::unique(keys.begin(), keys.end()), keys.end());
+    for (auto& k : keys)
+      if (k.empty()) throw Unsupported("a required pod (anti)affinity term with an empty topologyKey (an error in the reference, predicates.go:1311-1313)");
+    auto it = keysetID.find(keys);
+    if (it != keysetID.end()) return it->second;
+    const uint32_t s = (uint32_t)keysetID.size();
+    keysetID.emplace(keys, s);
+    std::map<std::vector<std::string>, int32_t> vals;
+    for (uint32_t n = 0; n < N; ++n) {
+      const api::Node& node = *ssn.Nodes.at(f.nodeNames[n])->node;
+      std::vector<std::string> v;
+      bool ok = true;
+      for (auto& k : keys) { auto l = node.Labels.find(k); if (l == node.Labels.end()) { ok = false; break; } v.push_back(l->second); }
+      pa.node_domain.push_back(ok ? vals.emplace(v, (int32_t)vals.size()).first->second : -1);
+    }
+    pa.keyset_domains.push_back((uint32_t)vals.size());
+    return s;
+  };
+
+  // ---- predicate groups ----
+  struct Group { uint32_t keyset; std::vector<bool> member; };   // member: by pod type
+  std::vector<Group> groups;
+  std::map<std::string, uint32_t> groupID;
+  auto addGroup = [&](const std::string& key, uint32_t keyset, const std::function<bool(const api::Pod&)>& member) {
+    auto it = groupID.find(key);
+    if (it != groupID.end()) return it->second;
+    const uint32_t g = (uint32_t)groups.size();
+    groupID.emplace(key, g);
+    Group gr{keyset, std::vector<bool>(reps.size())};
+    for (size_t ty = 0; ty < reps.size(); ++ty) gr.member[ty] = member(*reps[ty]);
+    groups.push_back(std::move(gr));
+    return g;
+  };
+  std::map<int, std::set<uint32_t>> forbid;           // pending type -> the groups it forbids
+  std::map<int, int32_t> need;
+  std::map<int, bool> selfMatch;
+  for (int ty : pendTypes) need[ty] = -1;
+  // (A) required anti-affinity terms pods own: satisfiesExistingPodsAntiAffinity (predicates.go:1400-1439)
+  std::set<int> owners(ltype.begin(), ltype.end());
+  owners.insert(pendTypes.begin(), pendTypes.end());
+  for (int oty : owners) {
+    const api::Pod& owner = *reps[oty];
+    for (auto& term : requiredTerms(owner, true)) {
+      if (term.TopologyKey.empty()) continue;         // node.Labels[""] never exists: the term rejects nothing (:1366)
+      const TermProps props = propsOf(owner, term);
+      std::vector<int> victims;
+      for (int ty : pendTypes) if (props.matches(*reps[ty])) victims.push_back(ty);
+      if (victims.empty()) continue;
+      const uint32_t ks = keysetOf({term.TopologyKey});
+      const std::string topo = term.TopologyKey, pkey = props.key;
+      const uint32_t g = addGroup("A|" + pkey + "|" + topo, ks, [&](const api::Pod& x) {
+        for (auto& t : requiredTerms(x, true)) {
+          if (t.TopologyKey != topo) continue;
+          try { if (propsOf(x, t).key == pkey) return true; } catch (const std::runtime_error&) {}   // an invalid term is no such term
+        }
+        return false;
+      });
+      for (int ty : victims) forbid[ty].insert(g);
+    }
+  }
+  // (B) the pending pods' own required terms: satisfiesPodsAffinityAntiAffinity, slow path (:1516-1562)
+  for (int ty : pendTypes) {
+    const api::Pod& pod = *reps[ty];
+    for (bool anti : {false, true}) {
+      const auto& ts = requiredTerms(pod, anti);
+      if (ts.empty()) continue;
+      std::vector<TermProps> props;
+      std::vector<std::string> keys, pkeys;
+      for (auto& t : ts) { props.push_back(propsOf(pod, t)); pkeys.push_back(props.back().key); keys.push_back(t.TopologyKey); }
+      const uint32_t ks = keysetOf(keys);
+      std::sort(pkeys.begin(), pkeys.end());
+      auto all = [&props](const api::Pod& x) {        // podMatchesAllAffinityTermProperties (metadata.go:601-612)
+        for (auto& p : props) if (!p.matches(x)) return false;
+        return true;
+      };
+      std::string gkey = "B|";
+      for (auto& k : pkeys) gkey += k + '\x02';
+      const uint32_t g = addGroup(gkey + "|" + std::to_string(ks), ks, all);
+      if (anti) forbid[ty].insert(g);
+      else { need[ty] = (int32_t)g; selfMatch[ty] = all(pod); }   // targetPodMatchesAffinityOfPod(pod, pod)
+    }
+  }
+  if (groups.size() > KB_MAX_AFF_GROUPS)
+    throw Unsupported(std::to_string(groups.size()) + " inter-pod affinity counter groups: more than KB_MAX_AFF_GROUPS (" + std::to_string(KB_MAX_AFF_GROUPS) + ")");
+  if (keysetID.size() > 64) throw Unsupported(std::to_string(keysetID.size()) + " topology key sets: more than 64");
+  const uint32_t NG = (uint32_t)groups.size();
+  pa.n_groups = NG;
+  std::vector<uint32_t> gOff(NG + 1, 0);
+  for (uint32_t g = 0; g < NG; ++g) { pa.group_keyset.push_back(groups[g].keyset); gOff[g + 1] = gOff[g] + pa.keyset_domains[groups[g].keyset]; }
+  pa.group_count0.assign(std::max(1u, gOff[NG]), 0);
+  pa.group_total0.assign(std::max(1u, NG), 0);
+  for (size_t i = 0; i < listed.size(); ++i) {
+    for (uint32_t g = 0; g < NG; ++g) {
+      if (!groups[g].member[ltype[i]]) continue;
+      pa.member_groups[listed[i].pod].push_back(g);
+      pa.group_total0[g]++;
+      const int32_t d = pa.node_domain[(size_t)groups[g].keyset * N + listed[i].node];
+      if (d >= 0) pa.group_count0[gOff[g] + d]++;
+    }
+  }
+
+  // ---- priority: weights between pod types (processPod, interpod_affinity.go:119-171), kinds, per-task lists ----
+  auto weights = [&](const api::Pod& in, const api::Pod& ex) {
+    std::map<std::string, int64_t> w;
+    auto add = [&](const api::Pod& owner, const api::PodAffinityTerm& term, const api::Pod& check, int64_t v) {
+      if (term.TopologyKey.empty() || v == 0) return;   // NodesHaveSameTopologyKey is false for an empty key
+      try { if (propsOf(owner, term).matches(check)) w[term.TopologyKey] += v; } catch (const std::runtime_error&) {}
+    };
+    for (auto& t : preferredTerms(in, false)) add(in, t.PodAffinityTerm, ex, t.Weight);
+    for (auto& t : preferredTerms(in, true)) add(in, t.PodAffinityTerm, ex, -(int64_t)t.Weight);
+    for (auto& t : requiredTerms(ex, false)) add(ex, t, in, 1);   // hardPodAffinityWeight = v1.DefaultHardPodAffinitySymmetricWeight (nodeorder.go:159)
+    for (auto& t : preferredTerms(ex, false)) add(ex, t.PodAffinityTerm, in, t.Weight);
+    for (auto& t : preferredTerms(ex, true)) add(ex, t.PodAffinityTerm, in, -(int64_t)t.Weight);
+    for (auto it = w.begin(); it != w.end();) it = it->second == 0 ? w.erase(it) : std::next(it);
+    return w;
+  };
+  std::map<std::pair<int, int>, std::map<std::string, int64_t>> wtab;
+  for (int pt : pendTypes) for (size_t xt = 0; xt < reps.size(); ++xt) wtab[{pt, (int)xt}] = weights(*reps[pt], *reps[xt]);
+  std::map<std::pair<std::vector<std::map<std::string, int64_t>>, bool>, int32_t> kindID;
+  std::vector<int> kindRep;
+  auto kindOf = [&](int xt, bool unbound) -> int32_t {
+    std::vector<std::map<std::string, int64_t>> vec;
+    bool nonzero = false;
+    for (int pt : pendTypes) { vec.push_back(wtab[{pt, xt}]); nonzero = nonzero || !vec.back().empty(); }
+    if (!nonzero) return -1;
+    auto ins = kindID.emplace(std::make_pair(vec, unbound), (int32_t)kindRep.size());
+    if (ins.second) { kindRep.push_back(xt); pa.kind_unbound.push_back(unbound ? 1 : 0); }
+    return ins.first->second;
+  };
+  std::vector<int32_t> xkind;
+  for (size_t i = 0; i < inTasks.size(); ++i) xkind.push_back(kindOf(ttype[i], inTasks[i].unbound));
+  std::map<int, int32_t> pkind;
+  for (int ty : pendTypes) pkind[ty] = kindOf(ty, true);   // a task placed in this session keeps an empty Spec.NodeName
+  pa.n_kinds = (uint32_t)kindRep.size();
+  pa.node_kind_count0.assign((size_t)std::max(1u, pa.n_kinds) * std::max(1u, N), 0);
+  for (size_t i = 0; i < inTasks.size(); ++i) if (xkind[i] >= 0) pa.node_kind_count0[(size_t)xkind[i] * N + inTasks[i].node]++;
+  struct WEntry { int32_t kind, keyset; int64_t value; };
+  std::map<int, std::vector<WEntry>> wlist;
+  for (int pt : pendTypes)
+    for (uint32_t k = 0; k < pa.n_kinds; ++k)
+      for (auto& kv : wtab[{pt, kindRep[k]}]) wlist[pt].push_back({(int32_t)k, (int32_t)keysetOf({kv.first}), kv.second});   // keys ascending
+  if (keysetID.size() > 64) throw Unsupported(std::to_string(keysetID.size()) + " topology key sets: more than 64");
+  pa.n_keysets = (uint32_t)keysetID.size();
+
+  // ---- per task ----
+  pa.task_forbid.assign(std::max(1u, T), 0); pa.task_contrib.assign(std::max(1u, T), 0);
+  pa.task_need.assign(std::max(1u, T), -1); pa.task_kind.assign(std::max(1u, T), -1);
+  pa.task_weight_off.assign(T + 1, 0);
+  if (NG > 64) pa.task_xgroup_off.assign(T + 1, 0);
+  for (uint32_t t = 0; t < T; ++t) {
+    const int ty = ptype[t];
+    pa.task_need[t] = need[ty];
+    pa.task_kind[t] = pkind[ty];
+    const std::set<uint32_t>& fb = forbid[ty];
+    for (uint32_t g = 0; g < NG; ++g) {               // groups < 64: bits of the masks; the others: entries of task_xgroup, ascending
+      const bool fg = fb.count(g) != 0, cg = groups[g].member[ty];
+      if (g < 64) {
+        if (fg) pa.task_forbid[t] |= 1ull << g;
+        if (cg) pa.task_contrib[t] |= 1ull << g;
+        continue;
+      }
+      if (fg || cg) pa.task_xgroup.push_back((g << 2) | (fg ? KB_XGROUP_FORBID : 0u) | (cg ? KB_XGROUP_CONTRIB : 0u));
+    }
+    if (!pa.task_xgroup_off.empty()) pa.task_xgroup_off[t + 1] = (uint32_t)pa.task_xgroup.size();
+    for (auto& e : wlist[ty]) { pa.weight_kind.push_back(e.kind); pa.weight_keyset.push_back(e.keyset); pa.weight_value.push_back(e.value); }
+    pa.task_weight_off[t + 1] = (uint32_t)pa.weight_kind.size();
+    if (hasPodAffinity(*f.tasks[t]->pod)) f.task_flags[t] |= KB_TASK_HAS_POD_AFFINITY;
+    if (selfMatch[ty]) f.task_flags[t] |= KB_TASK_AFF_SELF_MATCH;
+  }
+  // the arrays the engine reads need one element even when empty
+  if (pa.node_domain.empty()) pa.node_domain.assign(std::max(1u, N), 0);
+  if (pa.keyset_domains.empty()) pa.keyset_domains.push_back(0);
+  if (pa.group_keyset.empty()) pa.group_keyset.push_back(0);
+  if (pa.kind_unbound.empty()) pa.kind_unbound.push_back(0);
+  if (pa.weight_kind.empty()) { pa.weight_kind.push_back(0); pa.weight_keyset.push_back(0); pa.weight_value.push_back(0); }
+  if (pa.task_xgroup.empty()) pa.task_xgroup.push_back(0);
 }
 
 // One action on the GPU: flatten the session as it is NOW -> kb_session_load -> kb_allocate | kb_backfill -> replay the
@@ -650,6 +1122,22 @@ inline kb_snapshot SnapshotOf(Flat& f) {
   s.job_task_off = f.job_task_off.data(); s.job_min_avail = f.job_min_avail.data(); s.job_ready0 = f.job_ready0.data(); s.job_alloc0 = f.job_alloc0.data();
   s.job_alloc0_present = f.job_alloc0_present.data(); s.job_queue = f.job_queue.data(); s.job_prio = f.job_prio.data(); s.job_ctime = f.job_ctime.data();
   s.queue_weight = f.queue_weight.data(); s.queue_ctime = f.queue_ctime.data();
+  s.task_n_pref_terms = f.task_n_pref.data(); s.task_pref_terms = f.task_pref.data(); s.task_pref_weights = f.task_pref_w.data();
+  s.flags = f.snap_flags;
+  if (f.pa.on) {
+    Flat::PodAff& pa = f.pa;
+    kb_pod_affinity& c = pa.c;
+    c = kb_pod_affinity{};
+    c.n_keysets = pa.n_keysets; c.n_groups = pa.n_groups; c.n_kinds = pa.n_kinds; c.n_weights = pa.task_weight_off[f.T];
+    c.first_unbound_node = pa.first_unbound;
+    c.node_domain = pa.node_domain.data(); c.keyset_domains = pa.keyset_domains.data(); c.group_keyset = pa.group_keyset.data();
+    c.group_count0 = pa.group_count0.data(); c.group_total0 = pa.group_total0.data();
+    c.task_forbid = pa.task_forbid.data(); c.task_need = pa.task_need.data(); c.task_contrib = pa.task_contrib.data(); c.task_kind = pa.task_kind.data();
+    c.node_kind_count0 = pa.node_kind_count0.data(); c.kind_unbound = pa.kind_unbound.data(); c.task_weight_off = pa.task_weight_off.data();
+    c.weight_kind = pa.weight_kind.data(); c.weight_keyset = pa.weight_keyset.data(); c.weight_value = pa.weight_value.data();
+    if (!pa.task_xgroup_off.empty()) { c.task_xgroup_off = pa.task_xgroup_off.data(); c.task_xgroup = pa.task_xgroup.data(); }   // NULL when <= 64 groups
+    s.pod_affinity = &c;
+  }
   return s;
 }
 
@@ -722,11 +1210,13 @@ inline std::unique_ptr<framework::Action> New() { return std::make_unique<backfi
 // throws (no CPU fallback), in that shell and in every later shell of the same session.
 namespace actions { namespace cycle {
 
-// kb_running: the Running tasks of the session one by one (cycle.go::flattenRunning, builder.py meta["running"]).  No
-// inter-pod terms are flattened here, so no task is an affinity group member and aff_group_off / aff_group stay NULL.
+// kb_running: the Running tasks of the session one by one (cycle.go::flattenRunning, builder.py meta["running"] and
+// meta["running_aff_groups"]).  A task that is a member of a counter group of f.pa carries KB_RUNNING_AFF_MEMBER; its groups are
+// listed in aff_group_off / aff_group, which are always filled, so the engine keeps the member bits exact when it is evicted.
 struct Running {
   std::vector<std::shared_ptr<api::TaskInfo>> tasks;  // clones of the nodes' copies: what reclaim / preempt evict
   std::vector<uint32_t> node, job, present, uid_rank, flags;
+  std::vector<uint32_t> aff_group_off, aff_group;     // [n+1]; the groups, with one trailing 0 so that the array is never empty
   std::vector<double> resreq;                         // [R][n]
   std::vector<int32_t> prio, waiting;                 // waiting: [J]
   std::vector<int64_t> ctime;
@@ -751,7 +1241,7 @@ inline Running FlattenRunning(const framework::Session& ssn, const allocate::Fla
   for (auto& t : r.tasks) uids.push_back(t->UID);
   std::sort(uids.begin(), uids.end());
   r.node.assign(n1, 0); r.job = r.present = r.uid_rank = r.flags = r.node;
-  r.resreq.assign((size_t)f.R * n1, 0); r.prio.assign(n1, 0); r.ctime.assign(n1, 0);
+  r.resreq.assign((size_t)f.R * n1, 0); r.prio.assign(n1, 0); r.ctime.assign(n1, 0); r.aff_group_off.assign(n + 1, 0);
   for (uint32_t i = 0; i < n; ++i) {
     auto& t = *r.tasks[i];
     r.node[i] = nodeOf[i];
@@ -763,8 +1253,15 @@ inline Running FlattenRunning(const framework::Session& ssn, const allocate::Fla
       r.ctime[i] = t.pod->CreationTimestamp;
       const std::string& cn = t.pod->PriorityClassName;                    // conformance.go:45-53
       if (cn == "system-cluster-critical" || cn == "system-node-critical" || t.Namespace == "kube-system") r.flags[i] |= KB_RUNNING_CRITICAL;
+      auto m = f.pa.member_groups.find(t.pod.get());
+      if (m != f.pa.member_groups.end()) {              // its eviction takes it out of util.PodLister (kbgpu.h KB_RUNNING_AFF_MEMBER)
+        r.flags[i] |= KB_RUNNING_AFF_MEMBER;
+        r.aff_group.insert(r.aff_group.end(), m->second.begin(), m->second.end());
+      }
     }
+    r.aff_group_off[i + 1] = (uint32_t)r.aff_group.size();
   }
+  r.aff_group.push_back(0);
   r.waiting.assign(std::max<size_t>(1, f.jobIDs.size()), 0);
   for (uint32_t j = 0; j < f.jobIDs.size(); ++j) {     // WaitingTaskNum (job_info.go:396-405): 0 unless an earlier action pipelined tasks
     auto& idx = ssn.Jobs.at(f.jobIDs[j])->TaskStatusIndex;
@@ -819,7 +1316,11 @@ class Cycle : public std::enable_shared_from_this<Cycle> {
     run.node = rf.node.data(); run.job = rf.job.data(); run.resreq = rf.resreq.data(); run.res_present = rf.present.data();
     run.prio = rf.prio.data(); run.ctime = rf.ctime.data(); run.uid_rank = rf.uid_rank.data(); run.flags = rf.flags.data();
     run.job_waiting0 = rf.waiting.data();
-    allocate::Check(kb_session_load_running(e, &s, &run), "kb_session_load_running", e);
+    run.aff_group_off = rf.aff_group_off.data(); run.aff_group = rf.aff_group.data();
+    // only reclaim and preempt read the Running tasks: without them a session the victim walk cannot run is not refused
+    const bool evicts = std::find(actions_.begin(), actions_.end(), "reclaim") != actions_.end() ||
+                        std::find(actions_.begin(), actions_.end(), "preempt") != actions_.end();
+    if (evicts) allocate::Check(kb_session_load_running(e, &s, &run), "kb_session_load_running", e);
     std::vector<uint8_t> acts(actions_.size());
     for (size_t i = 0; i < actions_.size(); ++i) actionID(actions_[i], &acts[i]);
     dec_.assign(std::max(1u, flat_.T), kb_decision{});
