@@ -33,7 +33,7 @@ extern "C" {
 #define KB_MAX_W 4          /* 64-bit words per label / taint / host-port bitmask */
 #define KB_MAX_PREF_TERMS 4   /* preferred node-affinity terms per task */
 #define KB_MAX_AFF_TERMS 4  /* OR-ed required node-affinity terms carried per task */
-#define KB_MAX_Q 256        /* queues */
+#define KB_MAX_Q 65536      /* queues (kb_session_load refuses more with KB_E_BADARG) */
 
 typedef enum kb_status {
   KB_OK = 0,

@@ -19,7 +19,7 @@ KB_MAX_R = 8
 KB_MAX_W = 4
 KB_MAX_AFF_TERMS = 4
 KB_MAX_PREF_TERMS = 4
-KB_MAX_Q = 256
+KB_MAX_Q = 65536
 
 KB_OK = 0
 KB_E_BADARG = -1

@@ -214,7 +214,7 @@ inline bool hr_is_empty(uint32_t R, const HostRes& r) {                    // :9
 
 
 
-struct OffMut { size_t tiles, used, job_pos, job_ready, job_alloc, job_share, job_placed, q_head, dyn, q_alloc, q_share, qheap, dec, cand, ctl, sendbuf, recvbuf,
+struct OffMut { size_t tiles, used, job_pos, job_ready, job_alloc, job_share, job_placed, q_head, dyn, q_dyn, q_alloc, q_share, qheap, dec, cand, ctl, sendbuf, recvbuf,
                 bf_job_pos, bf_ctl, pipe_g, modlog, pcand, ppref, aff_cnt, aff_total, aff_kind_count, aff_first_unbound, aff_dom_sum, aff_minmax; };
 struct OffImm { size_t classes, ord_task, ord_class, ord_run, ord_peek, job_ord_off, job_min, job_queue, job_prio, job_tb, q_static, q_static_off, q_des, q_des_p, q_ctime, task_class, job_ready0,
                 bf_ord_task, bf_ord_class, bf_ord_run, bf_ord_peek, bf_job_ord_off, bf_jobs, bf_jobs_off, bf_classes, ord_chain, class_pref,
@@ -280,7 +280,7 @@ struct BuiltSession {
     D.job_pos = (uint32_t*)(mb + om.job_pos); D.job_ready = (int32_t*)(mb + om.job_ready);
     D.job_alloc = (double*)(mb + om.job_alloc); D.job_share = (double*)(mb + om.job_share);
     D.job_placed = (uint32_t*)(mb + om.job_placed); D.q_static_head = (uint32_t*)(mb + om.q_head);
-    D.dyn_jobs = (uint32_t*)(mb + om.dyn); D.q_allocated = (double*)(mb + om.q_alloc); D.q_share = (double*)(mb + om.q_share);
+    D.dyn_jobs = (uint32_t*)(mb + om.dyn); D.q_dyn_len = (uint32_t*)(mb + om.q_dyn); D.q_allocated = (double*)(mb + om.q_alloc); D.q_share = (double*)(mb + om.q_share);
     D.qheap = (uint32_t*)(mb + om.qheap); D.dec = (kb_decision*)(mb + om.dec); D.cand = (uint64_t*)(mb + om.cand);
     D.ctl = (Ctl*)(mb + om.ctl);
     D.tpi = tpi;
@@ -337,7 +337,7 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
   if (pa && pa->n_keysets > 64) return bfail(e, KB_E_UNSUPPORTED_FEATURE, "kb_pod_affinity: more than 64 key sets");
   if (s->flags & ~(KB_SNAPSHOT_PLACED_POD_AFFINITY | KB_SNAPSHOT_LISTED_POD_WITHOUT_NODE)) return bfail(e, KB_E_BADARG, "unknown kb_snapshot.flags bits 0x%x", s->flags);
   if (s->R < 2 || s->R > KB_MAX_R || s->W < 1 || s->W > KB_MAX_W) return bfail(e, KB_E_BADARG, "R=%u / W=%u out of range", s->R, s->W);
-  if (s->Q > KB_MAX_Q) return bfail(e, KB_E_BADARG, "Q=%u > KB_MAX_Q", s->Q);
+  if (s->Q > KB_MAX_Q) return bfail(e, KB_E_BADARG, "Q=%u > KB_MAX_Q (%u)", s->Q, (unsigned)KB_MAX_Q);
   if (s->N >= 0xFFFFFFF0u) return bfail(e, KB_E_BADARG, "N too large for the packed key");
   const uint32_t R = s->R, W = s->W, N = s->N, T = s->T, J = s->J, Q = s->Q;
   B.hc = HostConf();                 // a BuiltSession may be reused across loads (the engine keeps one to recycle its buffers)
@@ -824,6 +824,7 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
   om.job_placed = mut.alloc((size_t)std::max(1u, J) * 4);
   om.q_head = mut.alloc((size_t)std::max(1u, Q) * 4);
   om.dyn = mut.alloc((size_t)std::max(1u, J) * 4);
+  om.q_dyn = mut.alloc((size_t)std::max(1u, Q) * 4);
   om.q_alloc = mut.alloc((size_t)R * std::max(1u, Q) * 8);
   om.q_share = mut.alloc((size_t)std::max(1u, Q) * 8);
   om.qheap = mut.alloc((size_t)std::max(1u, J) * 4);
@@ -1031,26 +1032,29 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
       }
     }
     HostRes remaining = total;                                           // :100
-    std::vector<uint8_t> meet(Q, 0);
+    std::vector<uint32_t> active;                                        // used queues that have not met their request, ascending
+    for (uint32_t q = 0; q < Q; ++q) if (qa[q].used) active.push_back(q);
     for (;;) {
       int32_t totalWeight = 0;
-      for (uint32_t q = 0; q < Q; ++q) if (qa[q].used && !meet[q]) totalWeight += qa[q].weight;
+      for (const uint32_t q : active) totalWeight += qa[q].weight;
       if (totalWeight == 0) break;
       HostRes incD, decD;
-      for (uint32_t q = 0; q < Q; ++q) {
+      size_t keep = 0;
+      for (const uint32_t q : active) {
         Attr& a = qa[q];
-        if (!a.used || meet[q]) continue;
         HostRes old = a.deserved;
         HostRes part = remaining;
         const double ratio = (double)a.weight / (double)totalWeight;
         part.v[0] = part.v[0] * ratio; part.v[1] = part.v[1] * ratio;
         for (uint32_t k = 2; k < R; ++k) if ((part.present >> k) & 1u) part.v[k] = part.v[k] * ratio;
         hr_add(R, a.deserved, part);
-        if (hr_less(R, a.request, a.deserved)) { a.deserved = hr_min(R, a.deserved, a.request); meet[q] = 1; }
+        if (hr_less(R, a.request, a.deserved)) a.deserved = hr_min(R, a.deserved, a.request);
+        else active[keep++] = q;
         HostRes inc, dec;
         hr_diff(R, a.deserved, old, inc, dec);
         hr_add(R, incD, inc); hr_add(R, decD, dec);
       }
+      active.resize(keep);
       if (!hr_sub(R, remaining, incD)) return bfail(e, KB_E_STATE, "proportion: remaining.Sub would panic in the reference (resource_info.go:158)");
       hr_add(R, remaining, decD);
       if (hr_is_empty(R, remaining)) break;

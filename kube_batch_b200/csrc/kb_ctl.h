@@ -29,7 +29,6 @@ struct Ctl {
   uint32_t cur_class;     // class of the next run == class the next scan evaluates
   uint32_t cur_run;       // consecutive tasks of cur_class at the job's cursor
   uint32_t qheap_len;
-  uint32_t dyn_len;
   uint32_t step;          // next Allocate/Pipeline sequence number
   uint32_t tasks_processed, tasks_allocated, tasks_pipelined, visits, scans, rescans;
   uint32_t error;         // sticky: an invariant the reference would panic on
@@ -124,7 +123,8 @@ struct DevSession {
   uint32_t* q_static;     // [J] job ids sorted by initial JobOrderFn key, grouped by queue
   uint32_t* q_static_off; // [Q+1]
   uint32_t* q_static_head;// [Q]
-  uint32_t* dyn_jobs;     // [J] re-pushed jobs (allocate.go:186)
+  uint32_t* dyn_jobs;     // [J] re-pushed jobs (allocate.go:186), CSR by queue like q_static: queue q's at [q_static_off[q], + q_dyn_len[q])
+  uint32_t* q_dyn_len;    // [Q]
   // queues
   double*   q_deserved;   // [R][Q] proportion queueAttr.deserved
   uint32_t* q_deserved_present;
@@ -371,27 +371,26 @@ KB_HD void setup_run(const DevSession& S, Ctl& c) {
   c.cur_run = S.ord_run[pos];
 }
 
-// jobs.Pop() for queue q: minimum of {head of the static sorted list} U {re-pushed jobs of q}
-KB_HD int32_t pick_job(const DevSession& S, Ctl& c, uint32_t q) {
+// jobs.Pop() for queue q: minimum of {head of the static sorted list} U {re-pushed jobs of q}.  A queue's re-pushed jobs came
+// off its static list, so they fit in its q_static range; job_before is a strict total order, so the scan order does not matter.
+KB_HD int32_t pick_job(const DevSession& S, uint32_t q) {
   int32_t best = -1;
   int best_dyn = -1;
   uint32_t h = S.q_static_head[q];
   if (h < S.q_static_off[q + 1]) best = (int32_t)S.q_static[h];
-  for (uint32_t i = 0; i < c.dyn_len; ++i) {
-    uint32_t j = S.dyn_jobs[i];
-    if (S.job_queue[j] != q) continue;
+  uint32_t* dyn = S.dyn_jobs + S.q_static_off[q];
+  const uint32_t nd = S.q_dyn_len[q];
+  for (uint32_t i = 0; i < nd; ++i) {
+    uint32_t j = dyn[i];
     if (best < 0 || job_before(S, j, (uint32_t)best)) { best = (int32_t)j; best_dyn = (int)i; }
   }
   if (best < 0) return -1;
-  if (best_dyn >= 0) { S.dyn_jobs[best_dyn] = S.dyn_jobs[c.dyn_len - 1]; c.dyn_len -= 1; }
+  if (best_dyn >= 0) { dyn[best_dyn] = dyn[nd - 1]; S.q_dyn_len[q] = nd - 1; }
   else S.q_static_head[q] = h + 1;
   return best;
 }
-KB_HD bool queue_has_jobs(const DevSession& S, const Ctl& c, uint32_t q) {
-  if (S.q_static_head[q] < S.q_static_off[q + 1]) return true;
-  for (uint32_t i = 0; i < c.dyn_len; ++i)
-    if (S.job_queue[S.dyn_jobs[i]] == q) return true;
-  return false;
+KB_HD bool queue_has_jobs(const DevSession& S, uint32_t q) {
+  return S.q_static_head[q] < S.q_static_off[q + 1] || S.q_dyn_len[q] != 0;
 }
 
 // The outer `for {}` of allocate.go:89-193 from "queues.Pop()" until a job with tasks is found.
@@ -416,8 +415,8 @@ KB_HD void select_next_visit(const DevSession& S, Ctl& c) {
       if (c.qheap_len == 0) { c.done = 1; return; }                      // :90-92
       q = qheap_pop(S, c);                                                // :94
       if (queue_overused(S, q)) continue;                                 // :95-98
-      if (!queue_has_jobs(S, c, q)) continue;                             // :104-107
-      j = pick_job(S, c, q);                                              // :109
+      if (!queue_has_jobs(S, q)) continue;                                // :104-107
+      j = pick_job(S, q);                                                 // :109
       c.visits += 1;
       if (S.job_pos[j] >= S.job_ord_off[j + 1]) {                         // tasks.Empty(): the for at :129 is skipped
         qheap_push(S, c, q);                                              // :192
@@ -456,7 +455,8 @@ KB_HD void after_run(const DevSession& S, Ctl& c, uint32_t reason, uint32_t plac
   if (reason == STOP_NOFIT) end_visit = bf ? (S.job_pos[j] >= S.job_ord_off[j + 1])   // backfill.go:50-65: next task
                                                    : true;                                    // :144-148 break, job not re-pushed
   else if (reason == STOP_YIELD) {                                      // :185-188
-    S.dyn_jobs[c.dyn_len] = j; c.dyn_len += 1;
+    const uint32_t q = S.job_queue[j];
+    S.dyn_jobs[S.q_static_off[q] + S.q_dyn_len[q]] = j; S.q_dyn_len[q] += 1;
     end_visit = true;
   } else end_visit = S.job_pos[j] >= S.job_ord_off[j + 1];
   if (!end_visit) { setup_run(S, c); return; }
@@ -502,9 +502,10 @@ KB_HD void prep_allocate(const DevSession& S, Ctl& c, const uint32_t step0) {
       S.q_static[k] = v;
     }
     S.q_static_head[q] = lo;
+    S.q_dyn_len[q] = 0;
   }
   const uint32_t xe = c.xchg_epoch;
-  c.done = 0; c.cur_job = -1; c.qheap_len = 0; c.dyn_len = 0; c.error = 0;
+  c.done = 0; c.cur_job = -1; c.qheap_len = 0; c.error = 0;
   c.step = step0;
   for (uint32_t j = 0; j < S.J; ++j) qheap_push(S, c, S.job_queue[j]);      // one push PER JOB (allocate.go:52)
   select_next_visit<0>(S, c);

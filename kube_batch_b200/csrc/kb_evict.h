@@ -99,6 +99,7 @@ struct EvictDev {
   uint32_t* jheap;               // [J] job heaps of the queues (preemptorsMap), CSR by queue (S.q_static_off)
   uint32_t* jheap_len;           // [Q]
   uint32_t* qheap;               // [Q] reclaim's queue heap (each queue pushed once, reclaim.go:60-66)
+  uint32_t* queue_map;           // [Q] queueMap of reclaim.go:55 / preempt.go:58: the queue is in the heap already
   uint32_t* q_alloc_present;     // [Q] scalar presence of proportion's queueAttr.allocated
   uint32_t* evict_order;         // [n] by slot: order of the cache.Evict call, 0xFFFFFFFF = not evicted
   uint32_t* ops;                 // [n + Tall] Statement.operations: bit 31 = Pipeline(task), else Evict(slot)
@@ -551,10 +552,10 @@ KB_HD void evict_init(X& x, const DevSession& S, const EvictDev& E) {
     auto jless = [&](uint32_t l, uint32_t r) { return job_before(S, l, r); };
     ctl.qheap_len = 0; ctl.n_ops = 0; ctl.fail_valid = 0;
     ctl.fold_step = ctl.step;                                   // every Allocate of the cycle so far is in atom_cnt now
-    for (uint32_t q = 0; q < S.Q; ++q) { E.jheap_len[q] = 0; E.scratch[q] = 0; }    // scratch doubles as queueMap (Q <= KB_MAX_Q <= KB_EVICT_MAXV)
+    for (uint32_t q = 0; q < S.Q; ++q) { E.jheap_len[q] = 0; E.queue_map[q] = 0; }
     for (uint32_t j = 0; j < S.J; ++j) {
       const uint32_t q = S.job_queue[j];
-      if (!E.scratch[q]) { E.scratch[q] = 1; heap_push(E.qheap, ctl.qheap_len, q, qless); }
+      if (!E.queue_map[q]) { E.queue_map[q] = 1; heap_push(E.qheap, ctl.qheap_len, q, qless); }
       if (E.pt_pos[j] < E.pt_off[j + 1] - E.pt_off[j]) heap_push(E.jheap + S.q_static_off[q], E.jheap_len[q], j, jless);
     }
   }

@@ -14,7 +14,7 @@ struct EvictBuilt {
   Slab imm, mut;
   struct { size_t node_off, r_orig, r_job, r_resreq, r_present, r_prio, r_ctime, r_uid_rank, r_flags, pt_task, pt_off, task_class, task_present, job_waiting0,
                  r_atom_off, r_atom, atom_bit, atom_local; } oi;
-  struct { size_t r_state, pt_pos, job_waiting, jheap, jheap_len, qheap, q_alloc_present, evict_order, ops, scratch, ctl, atom_cnt; } om;
+  struct { size_t r_state, pt_pos, job_waiting, jheap, jheap_len, qheap, queue_map, q_alloc_present, evict_order, ops, scratch, ctl, atom_cnt; } om;
   uint32_t n_run = 0, Tall = 0;
   bool lists = false;                // kb_running carried aff_group_off: the atoms of the members are counted
   bool groups_unread = false;        // BuiltSession.aff_groups_unread: a member's eviction changes nothing observable (empty atom lists)
@@ -34,6 +34,7 @@ struct EvictBuilt {
     E.atom_cnt = (int32_t*)(mb + om.atom_cnt);
     E.r_state = (uint8_t*)(mb + om.r_state); E.pt_pos = (uint32_t*)(mb + om.pt_pos); E.job_waiting = (int32_t*)(mb + om.job_waiting);
     E.jheap = (uint32_t*)(mb + om.jheap); E.jheap_len = (uint32_t*)(mb + om.jheap_len); E.qheap = (uint32_t*)(mb + om.qheap);
+    E.queue_map = (uint32_t*)(mb + om.queue_map);
     E.q_alloc_present = (uint32_t*)(mb + om.q_alloc_present); E.evict_order = (uint32_t*)(mb + om.evict_order);
     E.ops = (uint32_t*)(mb + om.ops); E.scratch = (uint32_t*)(mb + om.scratch); E.ctl = (EvictCtl*)(mb + om.ctl);
   }
@@ -140,7 +141,7 @@ inline int build_evict(const kb_snapshot* s, const kb_running* run, const BuiltS
   EB.oi.r_atom_off = imm.alloc(((size_t)n + 1) * 4); EB.oi.r_atom = imm.alloc(std::max<size_t>(1, r_atom.size()) * 4);
   EB.oi.atom_bit = imm.alloc(std::max(1u, NA) * 4); EB.oi.atom_local = imm.alloc((size_t)64 * KB_MAX_W * 4);
   EB.om.r_state = mut.alloc(n1); EB.om.pt_pos = mut.alloc(J1 * 4); EB.om.job_waiting = mut.alloc(J1 * 4);
-  EB.om.jheap = mut.alloc(J1 * 4); EB.om.jheap_len = mut.alloc(Q1 * 4); EB.om.qheap = mut.alloc(Q1 * 4);
+  EB.om.jheap = mut.alloc(J1 * 4); EB.om.jheap_len = mut.alloc(Q1 * 4); EB.om.qheap = mut.alloc(Q1 * 4); EB.om.queue_map = mut.alloc(Q1 * 4);
   EB.om.q_alloc_present = mut.alloc(Q1 * 4); EB.om.evict_order = mut.alloc(n1 * 4);
   EB.om.ops = mut.alloc((n1 + T1) * 4); EB.om.scratch = mut.alloc((size_t)KB_EVICT_MAXV * 4); EB.om.ctl = mut.alloc(sizeof(EvictCtl));
   EB.om.atom_cnt = mut.alloc(std::max<size_t>(1, (size_t)NA * N) * 4);      // part of the pristine copy: every cycle starts from it

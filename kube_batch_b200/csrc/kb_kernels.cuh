@@ -574,6 +574,40 @@ __device__ __forceinline__ void load_ctl(Ctl& dst, const Ctl* g, int lane) {
   for (uint32_t i = lane; i < sizeof(Ctl) / 4; i += 32) d[i] = __ldcg(src + i);
 }
 
+// Several queues: the Go-heap emulation's next pop sifts down from the root and its next push climbs from the tail.  Pull the
+// top 12 levels of qheap (one load per line), the tail's ancestors, and the rows of the queues the first comparisons read: the
+// top 5 levels (31 entries) and the tail's ancestor chain — share, ctime, job-list cursors, deserved / allocated and, with HEAD,
+// the head job of their static lists — plus the re-pushed jobs of the root's queue.  At most three queue rows per lane per call,
+// whatever Q is.
+template <bool HEAD>
+__device__ __forceinline__ uint32_t prefetch_queue_heap(const DevSession& S, const uint32_t len, const int lane) {
+  const uint32_t R = S.cf.R;
+  uint32_t acc = 0;
+  for (uint32_t i = (uint32_t)lane * 32u; i < len && i < 4096u; i += 1024u) acc += S.qheap[i];
+  auto row = [&](const uint32_t qq) {
+    acc += (uint32_t)double_as_u64(S.q_share[qq]) + (uint32_t)S.q_ctime[qq] + S.q_static_head[qq] + S.q_static_off[qq + 1] + S.q_dyn_len[qq];
+    for (uint32_t k = 0; k < R; ++k)
+      acc += (uint32_t)double_as_u64(S.q_deserved[(size_t)k * S.Q + qq]) + (uint32_t)double_as_u64(S.q_allocated[(size_t)k * S.Q + qq]);
+    if (HEAD) {
+      const uint32_t hq = S.q_static_head[qq];
+      if (hq < S.q_static_off[qq + 1]) {
+        const uint32_t jn = S.q_static[hq];
+        const uint32_t pn = S.job_pos[jn];
+        acc += (uint32_t)S.job_ready[jn] + (uint32_t)S.job_min_avail[jn] + S.job_ord_off[jn + 1] + S.ord_class[pn] + S.ord_run[pn] + S.ord_task[pn];
+      }
+    }
+  };
+  if (lane < 31 && (uint32_t)lane < len) row(S.qheap[lane]);
+  const uint32_t up = ((len + 1) >> lane);                 // ancestors of the push position `len`
+  if (up >= 1 && up - 1 < len) row(S.qheap[up - 1]);
+  if (len) row(S.qheap[len - 1]);                          // moves to the root on the next pop
+  if (len) {
+    const uint32_t q0 = S.qheap[0];
+    if ((uint32_t)lane < S.q_dyn_len[q0]) acc += S.dyn_jobs[S.q_static_off[q0] + lane];
+  }
+  return acc;
+}
+
 // ---------------------------------------------------------------------------------------------
 // Shadow prefetch (warp 1 of the last CTA, concurrent with warp 0's gather / look-ahead / steps): touch the
 // job-level state of the current visit and what select_next_visit / setup_run will most likely read next (the head of
@@ -604,21 +638,7 @@ __device__ __forceinline__ void shadow_prefetch(const DevSession& S, const Ctl& 
     if (pn + lane < en) acc += S.ord_task[pn + lane];
     if ((uint32_t)lane < R) acc += (uint32_t)double_as_u64(S.job_alloc[(size_t)lane * S.J + jn]);
   }
-  if (S.Q > 1) {
-    // several queues: the Go-heap emulation walks qheap from the root (pop) and from the tail (push) and compares
-    // proportion shares; pull the first two levels-of-64, the tail's parent chain and every queue's share / deserved /
-    // allocated rows
-    const uint32_t len = c.qheap_len;
-    for (uint32_t i = (uint32_t)lane * 32u; i < len && i < 4096u; i += 1024u) acc += S.qheap[i];   // top 12 levels, one load per line
-    const uint32_t up = ((len + 1) >> lane);                 // ancestors of the push position `len`
-    if (up >= 1 && up - 1 < len) acc += S.qheap[up - 1];
-    for (uint32_t qq = lane; qq < S.Q; qq += 32) {
-      acc += (uint32_t)double_as_u64(S.q_share[qq]) + (uint32_t)S.q_ctime[qq] + S.q_static_head[qq] + S.q_static_off[qq + 1];
-      for (uint32_t k = 0; k < R; ++k)
-        acc += (uint32_t)double_as_u64(S.q_deserved[(size_t)k * S.Q + qq]) + (uint32_t)double_as_u64(S.q_allocated[(size_t)k * S.Q + qq]);
-    }
-    if ((uint32_t)lane < c.dyn_len) acc += S.dyn_jobs[lane];
-  }
+  if (S.Q > 1) acc += prefetch_queue_heap<false>(S, c.qheap_len, lane);
   acc = __reduce_add_sync(FULL, acc);
   if (lane == 0) *sink = acc;
 }

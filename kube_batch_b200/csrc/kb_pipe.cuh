@@ -889,25 +889,7 @@ __device__ __forceinline__ void pipe_shadow_warp(const DevSession& S, ReplaySmem
     }
     if ((uint32_t)lane < R) acc += (uint32_t)double_as_u64(S.q_allocated[(size_t)lane * S.Q + q]) + (uint32_t)double_as_u64(S.q_deserved[(size_t)lane * S.Q + q]);
     acc += S.q_deserved_present[q] + (uint32_t)double_as_u64(S.q_share[q]);
-    if (S.Q > 1) {
-      const uint32_t len = *((volatile uint32_t*)&sm.ctl.qheap_len);
-      for (uint32_t i = (uint32_t)lane * 32u; i < len && i < 4096u; i += 1024u) acc += S.qheap[i];
-      const uint32_t up = ((len + 1) >> lane);
-      if (up >= 1 && up - 1 < len) acc += S.qheap[up - 1];
-      for (uint32_t qq = lane; qq < S.Q; qq += 32) {
-        acc += (uint32_t)double_as_u64(S.q_share[qq]) + (uint32_t)S.q_ctime[qq] + S.q_static_head[qq] + S.q_static_off[qq + 1];
-        for (uint32_t k = 0; k < R; ++k)
-          acc += (uint32_t)double_as_u64(S.q_deserved[(size_t)k * S.Q + qq]) + (uint32_t)double_as_u64(S.q_allocated[(size_t)k * S.Q + qq]);
-        const uint32_t hq = S.q_static_head[qq];
-        if (hq < S.q_static_off[qq + 1]) {
-          const uint32_t jn = S.q_static[hq];
-          const uint32_t pn = S.job_pos[jn];
-          acc += (uint32_t)S.job_ready[jn] + (uint32_t)S.job_min_avail[jn] + S.job_ord_off[jn + 1] + S.ord_class[pn] + S.ord_run[pn] + S.ord_task[pn];
-        }
-      }
-      const uint32_t dl = *((volatile uint32_t*)&sm.ctl.dyn_len);
-      if ((uint32_t)lane < dl) acc += S.dyn_jobs[lane];
-    }
+    if (S.Q > 1) acc += prefetch_queue_heap<true>(S, *((volatile uint32_t*)&sm.ctl.qheap_len), lane);
   }
 }
 
