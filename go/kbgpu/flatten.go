@@ -68,10 +68,10 @@ type Flat struct {
 }
 
 const (
-	maxR         = 8 // KB_MAX_R
-	maxW         = 4 // KB_MAX_W
-	maxAffTerms  = 4 // KB_MAX_AFF_TERMS
-	maxPrefTerms = 4 // KB_MAX_PREF_TERMS
+	maxR         = 32 // KB_MAX_R
+	maxW         = 4  // KB_MAX_W
+	maxAffTerms  = 4  // KB_MAX_AFF_TERMS
+	maxPrefTerms = 4  // KB_MAX_PREF_TERMS
 )
 
 var builtin = map[string]bool{"priority": true, "gang": true, "drf": true, "predicates": true, "proportion": true,
@@ -317,7 +317,7 @@ func Flatten(ssn *framework.Session) (*Flat, error) {
 	}
 	R := len(f.Dims)
 	if R > maxR {
-		return nil, &ErrUnsupported{fmt.Sprintf("%d resource dimensions > KB_MAX_R", R)}
+		return nil, &ErrUnsupported{fmt.Sprintf("%d resource dimensions > KB_MAX_R (%d)", R, maxR)}
 	}
 
 	// ---- atoms ----

@@ -29,7 +29,7 @@ extern "C" {
 #define KB_ABI_VERSION 3u
 
 /* Compile-time capacity of the dense encodings. */
-#define KB_MAX_R 8          /* resource dims: 0 = cpu (milli), 1 = memory (bytes), 2.. = scalar resources (milli) */
+#define KB_MAX_R 32         /* resource dims: 0 = cpu (milli), 1 = memory (bytes), 2.. = scalar resources (milli); one bit per dim in the *_present masks */
 #define KB_MAX_W 4          /* 64-bit words per label / taint / host-port bitmask */
 #define KB_MAX_PREF_TERMS 4   /* preferred node-affinity terms per task */
 #define KB_MAX_AFF_TERMS 4  /* OR-ed required node-affinity terms carried per task */
@@ -165,7 +165,8 @@ typedef struct kb_pod_affinity {
  */
 typedef struct kb_snapshot {
   uint32_t abi_version;     /* KB_ABI_VERSION */
-  uint32_t R;               /* 2..KB_MAX_R */
+  uint32_t R;               /* 2..KB_MAX_R (> KB_MAX_R: KB_E_BADARG).  R <= 8 runs the 8-dimension kernel instances, 9..32 the
+                               32-dimension ones (wider class records and node tiles); R > 8 with KB_ENGINE_SHARD: KB_E_UNSUPPORTED_FEATURE */
   uint32_t W;               /* 1..KB_MAX_W */
   uint32_t N, T, J, Q;
   uint32_t flags;           /* KB_SNAPSHOT_* */

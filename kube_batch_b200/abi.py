@@ -15,7 +15,7 @@ KB_ENGINE_CHAIN4 = 1 << 4
 KB_ENGINE_NO_PIPE = 1 << 5
 KB_ENGINE_SHARD = 1 << 6
 KB_ABI_VERSION = 3
-KB_MAX_R = 8
+KB_MAX_R = 32
 KB_MAX_W = 4
 KB_MAX_AFF_TERMS = 4
 KB_MAX_PREF_TERMS = 4

@@ -219,7 +219,7 @@ struct OffMut { size_t tiles, used, job_pos, job_ready, job_alloc, job_share, jo
 struct OffImm { size_t classes, ord_task, ord_class, ord_run, ord_peek, job_ord_off, job_min, job_queue, job_prio, job_tb, q_static, q_static_off, q_des, q_des_p, q_ctime, task_class, job_ready0,
                 bf_ord_task, bf_ord_class, bf_ord_run, bf_ord_peek, bf_job_ord_off, bf_jobs, bf_jobs_off, bf_classes, ord_chain, class_pref,
                 aff_node_domain, aff_keyset_off, aff_group_keyset, aff_group_off, aff_cls, aff_w_kind, aff_w_keyset, aff_w_value, aff_kind_unbound,
-                aff_xf, aff_xc; };
+                aff_xf, aff_xc, total_hi; };
 
 struct BuiltSession {
   Slab mut, imm;
@@ -275,7 +275,8 @@ struct BuiltSession {
     for (int i = 0; i < 4; ++i) D.jobcmp[i] = hc.jobcmp[i];
     D.queue_order_proportion = hc.queue_order_proportion; D.proportion_present = hc.proportion_present; D.drf_present = hc.drf_present;
     D.total_dims_mask = total_dims_mask;
-    for (uint32_t r = 0; r < KB_MAX_R; ++r) D.total[r] = total[r];
+    for (uint32_t r = 0; r < KB_CLASS_R; ++r) D.total[r] = total[r];
+    D.total_hi = (const double*)(ib + oi.total_hi);
     D.tiles = (uint64_t*)(mb + om.tiles); D.node_used = (double*)(mb + om.used);
     D.job_pos = (uint32_t*)(mb + om.job_pos); D.job_ready = (int32_t*)(mb + om.job_ready);
     D.job_alloc = (double*)(mb + om.job_alloc); D.job_share = (double*)(mb + om.job_share);
@@ -320,12 +321,25 @@ struct BuiltSession {
 // evaluates preferred node affinity like the kernels do (counter path)
 inline bool allow_pref_legacy(bool allow_pref, uint32_t world) { return allow_pref && world > 1; }
 
+// Tiles per scan iteration of the per-visit kernels: up to 4 (16 warps), bounded by the shared memory left for the two staging
+// buffers next to VisitSmem — ~190 KB next to the narrow instances' ~26 KB, ~160 KB next to the wide instances' ~51 KB (class
+// record and candidate slots of up to 82 columns).  The widest record (R = 32, W = 4: 82 columns, 84 KB per tile) gets tpi = 1.
+inline uint32_t scan_tpi(const uint32_t R, const uint32_t W) {
+  const size_t tile_bytes = (size_t)tile_ncols(R, W) * TILE_NODES * 8;
+  const size_t budget = (R > KB_NARROW_R ? 160 : 190) * 1024;
+  uint32_t tpi = 4;
+  while (tpi > 1 && 2 * tpi * tile_bytes > budget) --tpi;
+  return tpi;
+}
+
 // Everything kb_session_load does before touching the device.  `max_grid` = scan CTAs (SM count).
 inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint32_t max_grid, BuiltSession& B, BuildErr* e,
                          uint32_t rank = 0, uint32_t world = 1, int overlap_mode = -1 /* -1 auto, 0 off, 1 on */,
                          uint32_t kchain = 1 /* classes per launch: 1, 2 or 4 (single GPU, no overlap) */,
                          bool allow_pref = false /* accept preferred node-affinity terms (tests/emu prototype only) */,
-                         int pipe_mode = 0 /* persistent pipeline (cycle_kernel): 0 off, 1 when the geometry allows it */) {
+                         int pipe_mode = 0 /* persistent pipeline (cycle_kernel): 0 off, 1 when the geometry allows it */,
+                         bool wide_classes = false /* the caller reads class tables of capacity KB_MAX_R (class_table<KB_MAX_R>):
+                                                      sessions with R > KB_CLASS_R are accepted (the engine's wide kernel instances) */) {
   if (!s) return bfail(e, KB_E_BADARG, "snapshot is NULL");
   if (s->abi_version != KB_ABI_VERSION) return bfail(e, KB_E_BADARG, "snapshot abi_version %u != %u", s->abi_version, KB_ABI_VERSION);
   const kb_pod_affinity* pa = s->pod_affinity;
@@ -336,7 +350,14 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
     return bfail(e, KB_E_UNSUPPORTED_FEATURE, "kb_pod_affinity: %u counter groups, more than %u", pa->n_groups, (unsigned)KB_MAX_AFF_GROUPS);
   if (pa && pa->n_keysets > 64) return bfail(e, KB_E_UNSUPPORTED_FEATURE, "kb_pod_affinity: more than 64 key sets");
   if (s->flags & ~(KB_SNAPSHOT_PLACED_POD_AFFINITY | KB_SNAPSHOT_LISTED_POD_WITHOUT_NODE)) return bfail(e, KB_E_BADARG, "unknown kb_snapshot.flags bits 0x%x", s->flags);
-  if (s->R < 2 || s->R > KB_MAX_R || s->W < 1 || s->W > KB_MAX_W) return bfail(e, KB_E_BADARG, "R=%u / W=%u out of range", s->R, s->W);
+  if (s->R < 2 || s->R > KB_MAX_R || s->W < 1 || s->W > KB_MAX_W)
+    return bfail(e, KB_E_BADARG, "R=%u / W=%u out of range (2 <= R <= KB_MAX_R = %u, 1 <= W <= KB_MAX_W = %u)", s->R, s->W, (unsigned)KB_MAX_R, (unsigned)KB_MAX_W);
+  if (s->R > KB_CLASS_R && !wide_classes)
+    return bfail(e, KB_E_BADARG, "R=%u: this build reads class records of %u resource dimensions (ClassRec)", s->R, (unsigned)KB_CLASS_R);
+  // the sharded exchange carries node records of at most KB_NARROW_R dimensions (P2P_RANK_U64)
+  if (world > 1 && s->R > KB_NARROW_R)
+    return bfail(e, KB_E_UNSUPPORTED_FEATURE, "R=%u resource dimensions with a sharded node axis (KB_ENGINE_SHARD): the exchange carries node records "
+                 "of at most %u dimensions", s->R, (unsigned)KB_NARROW_R);
   if (s->Q > KB_MAX_Q) return bfail(e, KB_E_BADARG, "Q=%u > KB_MAX_Q (%u)", s->Q, (unsigned)KB_MAX_Q);
   if (s->N >= 0xFFFFFFF0u) return bfail(e, KB_E_BADARG, "N too large for the packed key");
   const uint32_t R = s->R, W = s->W, N = s->N, T = s->T, J = s->J, Q = s->Q;
@@ -515,6 +536,13 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
         return bfail(e, KB_E_BADARG, "node %u: Idle is negative in dim %u (over-committed node: the reference cache would not produce it)", n, r);
     }
   std::vector<ClassRec> classes;
+  // dims KB_CLASS_R..R-1 of every class (initreq, then resreq; empty when R <= KB_CLASS_R): part of the class identity, joined
+  // with `classes` into the wide records of the class table
+  const uint32_t RH = R > KB_CLASS_R ? R - KB_CLASS_R : 0u;
+  std::vector<double> class_hi;
+  std::vector<double> hi(2 * (size_t)RH, 0.0);
+  auto init_of = [&](uint32_t id, uint32_t k) { return k < KB_CLASS_R ? classes[id].initreq[k] : class_hi[(size_t)id * 2 * RH + (k - KB_CLASS_R)]; };
+  auto same_hi = [&](uint32_t id) { return RH == 0 || memcmp(&class_hi[(size_t)id * 2 * RH], hi.data(), 2 * (size_t)RH * 8) == 0; };
   std::vector<ClassPref>& class_pref = B.class_pref;
   class_pref.clear(); B.has_pref = false;
   auto pref_of = [&](uint32_t t) {
@@ -662,9 +690,10 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
       ClassRec c;
       memset(&c, 0, sizeof c);
       for (uint32_t r = 0; r < R; ++r) {
-        c.initreq[r] = s->task_initreq[(size_t)r * T + t];
-        c.resreq[r] = s->task_resreq[(size_t)r * T + t];
-        if (c.resreq[r] > c.initreq[r]) return bfail(e, KB_E_BADARG, "task %u: resreq > initreq in dim %u (violates api/pod_info.go:53-73)", t, r);
+        const double ir = s->task_initreq[(size_t)r * T + t], rr = s->task_resreq[(size_t)r * T + t];
+        if (r < KB_CLASS_R) { c.initreq[r] = ir; c.resreq[r] = rr; }
+        else { hi[r - KB_CLASS_R] = ir; hi[RH + r - KB_CLASS_R] = rr; }
+        if (rr > ir) return bfail(e, KB_E_BADARG, "task %u: resreq > initreq in dim %u (violates api/pod_info.go:53-73)", t, r);
       }
       c.nz_cpu = s->task_nz_cpu[t]; c.nz_mem = s->task_nz_mem[t];
       c.n_aff = s->task_n_aff_terms[t];
@@ -680,21 +709,24 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
         if (hc.cf.predicates) atoms_of(pa_full->task_forbid[t], t, KB_XGROUP_FORBID, c.port_conflict);
         atoms_of(pa_full->task_contrib[t], t, KB_XGROUP_CONTRIB, c.aff_own);
       }
-      task_empty[t] = res_is_empty(R, [&](uint32_t k) { return c.resreq[k]; }) ? 1 : 0;   // allocate.go:113-118
-      if (prev_class != 0xFFFFFFFFu && memcmp(&classes[prev_class], &c, sizeof c) == 0 && memcmp(&class_pref[prev_class], &cp, sizeof cp) == 0) {
+      task_empty[t] = res_is_empty(R, [&](uint32_t k) { return k < KB_CLASS_R ? c.resreq[k] : hi[RH + k - KB_CLASS_R]; }) ? 1 : 0;   // allocate.go:113-118
+      if (prev_class != 0xFFFFFFFFu && memcmp(&classes[prev_class], &c, sizeof c) == 0 && memcmp(&class_pref[prev_class], &cp, sizeof cp) == 0 &&
+          same_hi(prev_class)) {
         task_class[t] = prev_class; continue; }
       uint64_t h = hash_rec(c);
       if (cp.n) { const uint64_t* w = reinterpret_cast<const uint64_t*>(&cp); for (size_t i = 0; i < sizeof(ClassPref) / 8; ++i) h = (h ^ w[i]) * 0xFF51AFD7ED558CCDull + (h >> 29); }
+      for (uint32_t i = 0; i < 2 * RH; ++i) { uint64_t u; memcpy(&u, &hi[i], 8); h = (h ^ u) * 0xFF51AFD7ED558CCDull + (h >> 29); }
       size_t mask = table.size() - 1, slot = (size_t)h & mask;
       uint32_t found = 0xFFFFFFFFu;
       while (table[slot] != 0xFFFFFFFFu) {
         const uint32_t id = table[slot];
-        if (class_hash[id] == h && memcmp(&classes[id], &c, sizeof c) == 0 && memcmp(&class_pref[id], &cp, sizeof cp) == 0) { found = id; break; }
+        if (class_hash[id] == h && memcmp(&classes[id], &c, sizeof c) == 0 && memcmp(&class_pref[id], &cp, sizeof cp) == 0 && same_hi(id)) { found = id; break; }
         slot = (slot + 1) & mask;
       }
       if (found == 0xFFFFFFFFu) {
         found = (uint32_t)classes.size();
         classes.push_back(c); class_pref.push_back(cp); class_hash.push_back(h);
+        class_hi.insert(class_hi.end(), hi.begin(), hi.end());
         table[slot] = found;
         if (classes.size() * 2 > table.size()) {            // grow + rehash
           std::vector<uint32_t> nt(table.size() * 4, 0xFFFFFFFFu);
@@ -707,7 +739,10 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
       prev_class = found;
     }
   }
-  if (classes.empty()) { ClassRec c; memset(&c, 0, sizeof c); classes.push_back(c); ClassPref cp; memset(&cp, 0, sizeof cp); class_pref.push_back(cp); }
+  if (classes.empty()) {
+    ClassRec c; memset(&c, 0, sizeof c); classes.push_back(c); ClassPref cp; memset(&cp, 0, sizeof cp); class_pref.push_back(cp);
+    class_hi.assign(2 * (size_t)RH, 0.0);
+  }
   static_assert(sizeof(ClassPref) % 8 == 0, "ClassPref is hashed as 64-bit words");
   if (B.has_pref) hc.cf.score_bias += 10ll * (hc.w_nodeaff < 0 ? -(int64_t)hc.w_nodeaff : 0);
   const uint32_t C = (uint32_t)classes.size();
@@ -765,8 +800,8 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
     bf_job_off[j] = (uint32_t)bf_task.size();
     const size_t b = bf_task.size();
     for (uint32_t t = s->job_task_off[j]; t < s->job_task_off[j + 1]; ++t) {
-      const ClassRec& c = classes[task_class[t]];
-      if (res_is_empty(R, [&](uint32_t k) { return c.initreq[k]; })) bf_task.push_back(t);
+      const uint32_t id = task_class[t];
+      if (res_is_empty(R, [&](uint32_t k) { return init_of(id, k); })) bf_task.push_back(t);
     }
     std::sort(bf_task.begin() + b, bf_task.end(), [&](uint32_t l, uint32_t r) { return s->task_uid_rank[l] < s->task_uid_rank[r]; });
     if (bf_task.size() > b) bf_jobs.push_back(j);
@@ -789,13 +824,7 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
   B.tile_lo = std::min(NT, rank * tiles_per_rank);
   B.tile_hi = std::min(NT, (rank + 1) * tiles_per_rank);
   B.nodes_per_rank = std::max(1u, tiles_per_rank * (uint32_t)TILE_NODES);
-  // tiles per scan iteration: up to 4 (16 warps), bounded by ~190 KB of shared memory for the two staging buffers
-  {
-    const size_t tile_bytes = (size_t)ncols * TILE_NODES * 8;
-    uint32_t tpi = 4;
-    while (tpi > 1 && 2 * tpi * tile_bytes > 190 * 1024) --tpi;
-    B.tpi = tpi;
-  }
+  B.tpi = scan_tpi(R, W);
   const uint32_t n_groups = (B.tile_hi - B.tile_lo + B.tpi - 1) / B.tpi;
   // overlap mode (one GPU) keeps one SM for the replayer CTA
   const uint32_t grid = std::max(1u, std::min(n_groups, GMAX > 1 ? GMAX - 1 : GMAX));   // one SM stays free for the replayer CTA
@@ -835,7 +864,9 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
   om.recvbuf = mut.alloc((size_t)std::max(1u, world) * xchg_u64(ncols) * 8);
   om.bf_job_pos = mut.alloc((size_t)std::max(1u, J) * 4);
   om.bf_ctl = mut.alloc(sizeof(Ctl));
-  oi.classes = imm.alloc((size_t)C * sizeof(ClassRec));
+  const size_t class_bytes = RH ? sizeof(ClassRecWide) : sizeof(ClassRec);
+  oi.classes = imm.alloc((size_t)C * class_bytes);
+  oi.total_hi = imm.alloc((size_t)std::max(1u, RH) * 8);
   oi.ord_task = imm.alloc((size_t)std::max(1u, To) * 4);
   oi.ord_class = imm.alloc((size_t)std::max(1u, To) * 4);
   oi.ord_run = imm.alloc((size_t)std::max(1u, To) * 4);
@@ -859,7 +890,7 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
   oi.bf_job_ord_off = imm.alloc((size_t)(J + 1) * 4);
   oi.bf_jobs = imm.alloc((size_t)std::max<size_t>(1, bf_jobs.size()) * 4);
   oi.bf_jobs_off = imm.alloc(2 * 4);
-  oi.bf_classes = imm.alloc((size_t)(Tb ? C : 1) * sizeof(ClassRec));
+  oi.bf_classes = imm.alloc((size_t)(Tb ? C : 1) * class_bytes);
   oi.ord_chain = imm.alloc((size_t)std::max(1u, To) * (KB_CHAIN_MAX - 1) * 4);
   oi.class_pref = imm.alloc((size_t)(B.has_pref ? C : 1) * sizeof(ClassPref));
   if (pa) {
@@ -923,7 +954,27 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
   }
 
   // ---------------- immutable job / queue / class tables ----------------
-  memcpy(H.classes, classes.data(), (size_t)C * sizeof(ClassRec));
+  // the class table in the session's capacity; a wide record joins the narrow part with its dims past KB_CLASS_R
+  auto write_classes = [&](unsigned char* dst, const bool backfill) {
+    for (uint32_t k = 0; k < C; ++k) {
+      if (!RH) {
+        ClassRec& d = reinterpret_cast<ClassRec*>(dst)[k];
+        d = classes[k];
+        if (backfill) for (uint32_t r = 0; r < KB_CLASS_R; ++r) d.initreq[r] = d.resreq[r];
+        continue;
+      }
+      ClassRecWide w;
+      memset(&w, 0, sizeof w);
+      class_copy(w, classes[k]);
+      for (uint32_t r = KB_CLASS_R; r < R; ++r) {
+        w.initreq[r] = class_hi[(size_t)k * 2 * RH + (r - KB_CLASS_R)];
+        w.resreq[r] = class_hi[(size_t)k * 2 * RH + RH + (r - KB_CLASS_R)];
+      }
+      if (backfill) for (uint32_t r = 0; r < KB_MAX_R; ++r) w.initreq[r] = w.resreq[r];
+      memcpy(dst + (size_t)k * sizeof(ClassRecWide), &w, sizeof w);
+    }
+  };
+  write_classes(imm.host.data() + oi.classes, false);
   if (B.has_pref) memcpy(imm.host.data() + oi.class_pref, class_pref.data(), (size_t)C * sizeof(ClassPref));
   if (pa) {
     unsigned char* ib = imm.host.data(); unsigned char* mb = mut.host.data();
@@ -1001,16 +1052,22 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
 
   // drf OnSessionOpen (drf.go:60-83): total = sum of node Allocatable; share per job
   H.total_dims_mask = 3u;
-  for (uint32_t r = 0; r < R; ++r) H.total[r] = 0;
+  for (uint32_t r = 0; r < KB_MAX_R; ++r) B.total[r] = 0;
   for (uint32_t n = 0; n < N; ++n) {
     H.total_dims_mask |= s->node_alloc_present[n] & ~3u;
     for (uint32_t r = 0; r < R; ++r)
-      if (r < 2 || ((s->node_alloc_present[n] >> r) & 1u)) H.total[r] += s->node_allocatable[(size_t)r * N + n];
+      if (r < 2 || ((s->node_alloc_present[n] >> r) & 1u)) B.total[r] += s->node_allocatable[(size_t)r * N + n];
   }
   H.total_dims_mask &= (R >= 32 ? 0xFFFFFFFFu : ((1u << R) - 1u));
   B.total_dims_mask = H.total_dims_mask;
-  for (uint32_t r = 0; r < KB_MAX_R; ++r) B.total[r] = H.total[r];
-  for (uint32_t j = 0; j < J; ++j) { if (hc.drf_present) update_job_share(H, j); else H.job_share[j] = 0.0; }
+  for (uint32_t r = 0; r < R && r < KB_CLASS_R; ++r) H.total[r] = B.total[r];
+  if (KB_CLASS_R < KB_MAX_R)
+    for (uint32_t i = 0; i < RH; ++i) reinterpret_cast<double*>(imm.host.data() + oi.total_hi)[i] = B.total[KB_CLASS_R + i];
+  for (uint32_t j = 0; j < J; ++j) {
+    if (!hc.drf_present) H.job_share[j] = 0.0;
+    else if (RH) update_job_share<KB_MAX_R>(H, j);
+    else update_job_share(H, j);
+  }
 
   // proportion OnSessionOpen (proportion.go:58-154)
   B.q_alloc_present.assign(std::max(1u, Q), 0);
@@ -1018,7 +1075,7 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
     struct Attr { bool used = false; int32_t weight = 0; HostRes deserved, allocated, request; };
     std::vector<Attr> qa(Q);
     HostRes total; total.present = H.total_dims_mask & ~3u;
-    for (uint32_t r = 0; r < R; ++r) total.v[r] = H.total[r];
+    for (uint32_t r = 0; r < R; ++r) total.v[r] = B.total[r];
     for (uint32_t j = 0; j < J; ++j) {                                   // :67-98
       Attr& a = qa[s->job_queue[j]];
       if (!a.used) { a.used = true; a.weight = s->queue_weight[s->job_queue[j]]; }
@@ -1139,10 +1196,7 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
   {
     DevSession HB{};
     B.bind_backfill(HB, mut.host.data(), imm.host.data());
-    if (Tb) {
-      memcpy(HB.classes, classes.data(), (size_t)C * sizeof(ClassRec));
-      for (uint32_t k = 0; k < C; ++k) for (uint32_t r = 0; r < KB_MAX_R; ++r) HB.classes[k].initreq[r] = HB.classes[k].resreq[r];
-    }
+    if (Tb) write_classes(imm.host.data() + oi.bf_classes, true);
     for (uint32_t i = 0; i < Tb; ++i) { HB.ord_task[i] = bf_task[i]; HB.ord_class[i] = task_class[bf_task[i]]; HB.ord_peek[i] = 0xFFFFFFFFu; }
     for (uint32_t j = 0; j < J; ++j) {
       for (uint32_t i = bf_job_off[j + 1]; i-- > bf_job_off[j];)

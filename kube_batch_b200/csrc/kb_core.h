@@ -80,9 +80,17 @@ struct EvalConf {
 
 // One task equivalence class: every field of a pending task that predicateFn / the prioritizers /
 // AddTask read.  Tasks of a PodGroup are normally one class.
-struct ClassRec {
-  double   initreq[KB_MAX_R];
-  double   resreq[KB_MAX_R];
+//
+// RC: resource dimensions the record holds (its class capacity).  A session with R <= KB_NARROW_R uses the narrow record
+// ClassRecT<KB_NARROW_R> — the layout tests/probe mirrors — and the kernels' narrow instances; a session with up to KB_MAX_R
+// dimensions uses ClassRecT<KB_MAX_R> and the wide instances (the kernels take RC as a template parameter and read the class
+// table through class_table<RC>).  Dimensions >= R are 0.
+constexpr uint32_t KB_NARROW_R = 8;
+template <uint32_t RC>
+struct ClassRecT {
+  static constexpr uint32_t CAP = RC;
+  double   initreq[RC];
+  double   resreq[RC];
   int64_t  nz_cpu, nz_mem;
   uint64_t sel_req[KB_MAX_W];
   uint64_t aff[KB_MAX_AFF_TERMS][KB_MAX_W];
@@ -94,6 +102,27 @@ struct ClassRec {
   uint32_t n_aff;
   uint32_t flags;             // KB_TASK_BEST_EFFORT_QOS only
 };
+// KB_CLASS_R: the capacity of `ClassRec`, i.e. of host code that reads DevSession.classes as ClassRec (the session builder, the
+// evict walk's CPU policy, tests/emu).  The library is built with KB_NARROW_R; tests/emu_wide builds the emulation with KB_MAX_R.
+#ifndef KB_CLASS_R
+#define KB_CLASS_R 8
+#endif
+static_assert(KB_CLASS_R == KB_NARROW_R || KB_CLASS_R == KB_MAX_R, "KB_CLASS_R is the narrow or the full capacity");
+using ClassRec = ClassRecT<KB_CLASS_R>;
+using ClassRecWide = ClassRecT<KB_MAX_R>;
+
+// Copies a class record into a record of another capacity (dimensions the destination holds beyond the source's become 0)
+template <uint32_t A, uint32_t B>
+inline void class_copy(ClassRecT<A>& d, const ClassRecT<B>& s) {
+  for (uint32_t k = 0; k < A; ++k) { d.initreq[k] = k < B ? s.initreq[k] : 0.0; d.resreq[k] = k < B ? s.resreq[k] : 0.0; }
+  d.nz_cpu = s.nz_cpu; d.nz_mem = s.nz_mem;
+  for (uint32_t w = 0; w < KB_MAX_W; ++w) {
+    d.sel_req[w] = s.sel_req[w]; d.tol[w] = s.tol[w]; d.port_own[w] = s.port_own[w]; d.port_conflict[w] = s.port_conflict[w];
+    d.aff_own[w] = s.aff_own[w];
+    for (uint32_t t = 0; t < KB_MAX_AFF_TERMS; ++t) d.aff[t][w] = s.aff[t][w];
+  }
+  d.n_aff = s.n_aff; d.flags = s.flags;
+}
 
 // Preferred node-affinity terms of a class (NodeAffinityPriority, vendor/.../priorities/node_affinity.go:34-77): requirement
 // atoms that must ALL hold on the node + the term's weight.  Evaluated by cycle_kernel (two-pass scan, kb_pipe.cuh), the
@@ -211,8 +240,8 @@ KB_HD uint32_t key_node(uint64_t key) { return 0xFFFFFFFFu - (uint32_t)(key & 0x
 KB_HD int64_t key_score(uint64_t key) { return (int64_t)(key >> 32); }
 
 // K2 alone: the biased weighted sum of the Map priorities for one (class, node) pair (util/scheduler_helper.go:162-168)
-template <class NodeAcc>
-KB_HD int64_t node_score(const EvalConf& cf, const ClassRec& c, const NodeAcc& n) {
+template <class NodeAcc, class CR>
+KB_HD int64_t node_score(const EvalConf& cf, const CR& c, const NodeAcc& n) {
   int64_t score = cf.score_bias;
   if (cf.nodeorder) {
     // resource_allocation.go:100-123: req = nodeInfo.NonZeroRequest() + pod non-zero request
@@ -234,8 +263,8 @@ KB_HD int64_t node_score(const EvalConf& cf, const ClassRec& c, const NodeAcc& n
 // ssn.PredicateFn alone — backfill needs it to reproduce ssn.Allocate's status-before-AddTask order (session.go:241-262).
 // RR / WW: compile-time copies of cf.R / cf.W (0 = read them at run time).  The kernels instantiate the common geometry
 // (R = 3, W = 2) so that every loop below unrolls into straight-line code; semantics are identical.
-template <int RR = 0, int WW = 0, class NodeAcc>
-KB_HD uint64_t eval_pair(const EvalConf& cf, const ClassRec& c, const NodeAcc& n, uint32_t node_idx, bool* fits_idle, bool* pred_ok = nullptr) {
+template <int RR = 0, int WW = 0, class NodeAcc, class CR>
+KB_HD uint64_t eval_pair(const EvalConf& cf, const CR& c, const NodeAcc& n, uint32_t node_idx, bool* fits_idle, bool* pred_ok = nullptr) {
   // Written branch-free on purpose: a lone warp (the replay) or one warp per SM sub-partition (the scan)
   // hides latency only through instruction-level parallelism, so every check is computed and AND-ed.
   const uint32_t R = RR ? (uint32_t)RR : cf.R, W = WW ? (uint32_t)WW : cf.W;

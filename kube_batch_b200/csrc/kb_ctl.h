@@ -93,7 +93,7 @@ struct DevSession {
   uint32_t queue_order_proportion;
   uint32_t proportion_present, drf_present;
   uint32_t total_dims_mask;            // dims of drf totalResource.ResourceNames()
-  double   total[KB_MAX_R];            // sum of node Allocatable (drf.go:62-64)
+  double   total[KB_CLASS_R];          // sum of node Allocatable (drf.go:62-64), dims 0..KB_CLASS_R-1; the rest in total_hi
   // node table: NT tiles of [ncols][TILE_NODES] u64, see tile_col_* below
   uint64_t* tiles;
   double*   node_used;    // [R][N] bookkeeping only
@@ -160,9 +160,21 @@ struct DevSession {
   uint32_t pad_pref;
   uint32_t* dbg;          // 64 progress words in mapped host memory (KB_PIPE_DEBUG=1; NULL otherwise): read by the host watchdog when a cycle hangs
   AffDev aff;             // inter-pod (anti)affinity tables and counters (kb_aff.h); aff.on == 0: the session carries none
+  const double* total_hi; // [R - KB_CLASS_R] dims KB_CLASS_R.. of `total` (sessions with more dims than ClassRec holds), next to the
+                          // wide class table in the immutable slab; read through total_of
 };
+// The class table as records of capacity RC (ClassRecT): RC == KB_CLASS_R for a session with R <= KB_CLASS_R, KB_MAX_R above
+template <uint32_t RC>
+KB_HD const ClassRecT<RC>* class_table(const DevSession& S) { return reinterpret_cast<const ClassRecT<RC>*>(S.classes); }
+// drf's totalResource in dimension k (k < R) of a session whose class capacity is RC
+template <uint32_t RC = KB_CLASS_R>
+KB_HD double total_of(const DevSession& S, const uint32_t k) {
+  if (RC <= KB_CLASS_R) return S.total[k];
+  return k < KB_CLASS_R ? S.total[k] : S.total_hi[k - KB_CLASS_R];
+}
 constexpr uint32_t KB_MAX_WORLD = 8;
-constexpr uint32_t P2P_RANK_U64 = (2 + 2 * KB_MAX_R + 6 + 3 * KB_MAX_W) * 32;         // keys + widest record block + flag row
+constexpr uint32_t P2P_RANK_U64 = (2 + 2 * KB_NARROW_R + 6 + 3 * KB_MAX_W) * 32;      // keys + widest record block + flag row
+                                                                                      // (the sharded path takes R <= KB_NARROW_R only)
 constexpr uint32_t P2P_FLAG_OFF = 2 * KB_MAX_WORLD * P2P_RANK_U64;
 constexpr size_t   P2P_REGION_BYTES = ((size_t)P2P_FLAG_OFF + 2 * KB_MAX_WORLD) * 8;
 
@@ -325,11 +337,12 @@ KB_HD uint32_t qheap_pop(const DevSession& S, Ctl& c) {
 // plugin bookkeeping
 // ---------------------------------------------------------------------------------------------
 // drf.calculateShare (drf.go:161-171)
+template <uint32_t RC = KB_CLASS_R>
 KB_HD void update_job_share(const DevSession& S, uint32_t j) {
   double res = 0;
   for (uint32_t k = 0; k < S.cf.R; ++k) {
     if (!((S.total_dims_mask >> k) & 1u)) continue;
-    double sh = share_of(S.job_alloc[(size_t)k * S.J + j], S.total[k]);
+    double sh = share_of(S.job_alloc[(size_t)k * S.J + j], total_of<RC>(S, k));
     if (sh > res) res = sh;
   }
   S.job_share[j] = res;
@@ -354,7 +367,8 @@ KB_HD bool queue_overused(const DevSession& S, uint32_t q) {
 }
 
 // AllocateFunc event handlers of drf (drf.go:136-144) and proportion (proportion.go:213-222) for one placed task
-KB_HD void on_allocate_event(const DevSession& S, uint32_t j, const ClassRec& c) {
+template <class CR>
+KB_HD void on_allocate_event(const DevSession& S, uint32_t j, const CR& c) {
   const uint32_t q = S.job_queue[j];
   for (uint32_t k = 0; k < S.cf.R; ++k) {
     if (S.drf_present) S.job_alloc[(size_t)k * S.J + j] = KB_DADD(S.job_alloc[(size_t)k * S.J + j], c.resreq[k]);
@@ -441,13 +455,13 @@ KB_HD void publish_chain(const DevSession& S, Ctl& c) {
 
 // Called once a run stopped.  `placed` = tasks of the run that went through Allocate/Pipeline.
 // shares_done: the caller already refreshed the job's drf share and the queue's proportion share (the replay warp does
-// the divisions of all dimensions in parallel lanes)
-template <int BF = -1>
+// the divisions of all dimensions in parallel lanes).  RC: class capacity of the session (drf's totals past KB_CLASS_R, total_of)
+template <int BF = -1, uint32_t RC = KB_CLASS_R>
 KB_HD void after_run(const DevSession& S, Ctl& c, uint32_t reason, uint32_t placed, const bool shares_done = false) {
   const bool bf = BF < 0 ? S.backfill != 0 : BF != 0;
   const uint32_t j = (uint32_t)c.cur_job;
   if (placed && !shares_done) {
-    if (S.drf_present) update_job_share(S, j);
+    if (S.drf_present) update_job_share<RC>(S, j);
     if (S.proportion_present) update_queue_share(S, S.job_queue[j]);
   }
   if (reason == STOP_RESCAN) { setup_run(S, c); return; }

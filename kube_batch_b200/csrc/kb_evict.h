@@ -17,6 +17,9 @@
 #ifndef KB_EVICT_H_
 #define KB_EVICT_H_
 
+#include <type_traits>
+#include <utility>
+
 #include "kb_ctl.h"
 
 namespace kb {
@@ -62,7 +65,10 @@ struct EvictCtl {
   unsigned long long red;
   long long amin, amax;            // workers -> master (pass 4): min / max InterPodAffinityPriority count; master -> workers (sweep)
   Preemptor pre;
-  ClassRec cls;
+  union {                          // master -> workers: the preemptor's class record, in the capacity of the kernel instance
+    ClassRec cls;
+    ClassRecWide cls_wide;
+  };
 };
 
 // Device view of the evict path's own data (everything else — node tiles, job / queue accounting, classes — is the
@@ -129,12 +135,14 @@ KB_HD bool res_less(uint32_t R, LAcc l, uint32_t lp, RAcc r, uint32_t rp) {
   return true;
 }
 
-// drf.calculateShare (drf.go:161-171) of an allocation vector
+// drf.calculateShare (drf.go:161-171) of an allocation vector.  RC: class capacity of the session (ClassRecT), which also
+// sizes the local resource vectors of the walk below
+template <uint32_t RC>
 KB_HD double drf_share_of(const DevSession& S, const double* alloc) {
   double res = 0;
   for (uint32_t k = 0; k < S.cf.R; ++k) {
     if (!((S.total_dims_mask >> k) & 1u)) continue;
-    const double sh = share_of(alloc[k], S.total[k]);
+    const double sh = share_of(alloc[k], total_of<RC>(S, k));
     if (sh > res) res = sh;
   }
   return res;
@@ -154,6 +162,7 @@ KB_HD bool evict_candidate(const DevSession& S, const EvictDev& E, const Preempt
 
 // One candidate through the deciding tier's filters.  `lo` = first slot of the node: drf / proportion subtract the
 // candidates BEFORE this one (same job / same queue) cumulatively, in list order, exactly like the cloned allocations map.
+template <uint32_t RC>
 KB_HD bool evict_is_victim(const DevSession& S, const EvictDev& E, const Preemptor& P, const uint32_t fns, const uint32_t lo, const uint32_t slot, uint32_t* err) {
   const uint32_t R = S.cf.R, n = E.n_run;
   const uint32_t j = E.r_job[slot];
@@ -165,19 +174,19 @@ KB_HD bool evict_is_victim(const DevSession& S, const EvictDev& E, const Preempt
   if (fns & EVF_PRIORITY) v = v && !(S.job_prio[j] >= S.job_prio[P.job]);       // priority.go:81-100
   if (fns & EVF_CONFORMANCE) v = v && !(E.r_flags[slot] & 1u);                   // conformance.go:45-58
   if (fns & EVF_DRF) {                                           // drf.go:90-107
-    double ralloc[KB_MAX_R];
+    double ralloc[RC];
     for (uint32_t k = 0; k < R; ++k) ralloc[k] = S.job_alloc[(size_t)k * S.J + j];
     for (uint32_t s2 = lo; s2 <= slot; ++s2) {
       if (E.r_job[s2] != j || !evict_candidate(S, E, P, s2)) continue;
       if (!res_less_equal(R, [&](uint32_t k) { return E.r_resreq[(size_t)k * n + s2]; }, [&](uint32_t k) { return ralloc[k]; })) { *err = 1; return false; }
       for (uint32_t k = 0; k < R; ++k) ralloc[k] = KB_DSUB(ralloc[k], E.r_resreq[(size_t)k * n + s2]);
     }
-    const double rs = drf_share_of(S, ralloc);
+    const double rs = drf_share_of<RC>(S, ralloc);
     v = v && (P.ls < rs || KB_FABS(KB_DSUB(P.ls, rs)) <= 0.000001);
   }
   if (fns & EVF_PROPORTION) {                                    // proportion.go:171-196
     const uint32_t q = S.job_queue[j];
-    double al[KB_MAX_R];
+    double al[RC];
     for (uint32_t k = 0; k < R; ++k) al[k] = S.q_allocated[(size_t)k * S.Q + q];
     const uint32_t ap = E.q_alloc_present[q];
     bool mine = false;
@@ -209,7 +218,8 @@ KB_HD const ClassAff* evict_aff(const DevSession& S, const Preemptor& P) {
 }
 
 // ssn.PredicateFn (K1 without the Idle test: preempt never checks Idle) on one node
-KB_HD bool evict_pred_ok(const DevSession& S, const ClassRec& c, const uint32_t node) {
+template <class CR>
+KB_HD bool evict_pred_ok(const DevSession& S, const CR& c, const uint32_t node) {
   const size_t tile_u64 = (size_t)S.ncols * TILE_NODES;
   TileAcc acc{S.tiles + (size_t)(node / TILE_NODES) * tile_u64, node % TILE_NODES, S.cf.R, S.cf.W};
   bool pok = true;
@@ -221,7 +231,8 @@ KB_HD bool evict_pred_ok(const DevSession& S, const ClassRec& c, const uint32_t 
 // NormalizeReduce divides by the max count over util.PredicateNodes (preempt.go:180-189, reduce.go:28-63), i.e. over EVERY node
 // that passes the predicates — also nodes without Running tasks or eligible victims, and full nodes (preempt never checks Idle) —
 // so this runs on all nodes, not only on those evict_node_key gives a key.  The max starts at 0, so 0 stands for "not counted".
-KB_HD uint32_t evict_pref_count(const DevSession& S, const ClassRec& c, const ClassPref& cp, const uint32_t node) {
+template <class CR>
+KB_HD uint32_t evict_pref_count(const DevSession& S, const CR& c, const ClassPref& cp, const uint32_t node) {
   if (!evict_pred_ok(S, c, node)) return 0;
   const size_t tile_u64 = (size_t)S.ncols * TILE_NODES;
   TileAcc acc{S.tiles + (size_t)(node / TILE_NODES) * tile_u64, node % TILE_NODES, S.cf.R, S.cf.W};
@@ -245,7 +256,8 @@ struct EvictPrio {
 // K1 (+K2 for preempt) + the victim walk of one node: packed key (score, node) if the node's victims cover InitResreq, else 0.
 // The score gains nodeaffinity.weight * (10 * count / pmax) and podaffinity.weight * aff_score (negative weights are already
 // folded into cf.score_bias).
-KB_HD uint64_t evict_node_key(const DevSession& S, const EvictDev& E, const Preemptor& P, const ClassRec& c, const EvictPrio& pr,
+template <class CR>
+KB_HD uint64_t evict_node_key(const DevSession& S, const EvictDev& E, const Preemptor& P, const CR& c, const EvictPrio& pr,
                               const uint32_t node, uint32_t* err) {
   const uint32_t R = S.cf.R, W = S.cf.W, n = E.n_run;
   const uint32_t lo = E.node_off[node], hi = E.node_off[node + 1];
@@ -258,12 +270,12 @@ KB_HD uint64_t evict_node_key(const DevSession& S, const EvictDev& E, const Pree
   if (!pok) return 0;
   const uint32_t fns = P.mode == 0 ? E.ec.reclaim_fns : E.ec.preempt_fns;
   if (fns == 0) return 0;                                                  // no plugin registered a filter: victims == nil
-  double all[KB_MAX_R];
+  double all[CR::CAP];
   for (uint32_t k = 0; k < R; ++k) all[k] = 0.0;
   uint32_t nv = 0;
   for (uint32_t s = lo; s < hi; ++s) {
     if (!evict_candidate(S, E, P, s)) continue;
-    if (!evict_is_victim(S, E, P, fns, lo, s, err)) continue;
+    if (!evict_is_victim<CR::CAP>(S, E, P, fns, lo, s, err)) continue;
     for (uint32_t k = 0; k < R; ++k) all[k] = KB_DADD(all[k], E.r_resreq[(size_t)k * n + s]);
     ++nv;
   }
@@ -278,6 +290,7 @@ KB_HD uint64_t evict_node_key(const DevSession& S, const EvictDev& E, const Pree
 
 // ---- state changes (thread 0) ----
 // Session.Evict / Statement.Evict without the cache call: UpdateTaskStatus(Releasing), node.UpdateTask, DeallocateFunc handlers
+template <uint32_t RC>
 KB_HD void evict_apply(const DevSession& S, const EvictDev& E, const uint32_t node, const uint32_t slot, const bool undo) {
   const uint32_t R = S.cf.R, n = E.n_run;
   const uint32_t j = E.r_job[slot], q = S.job_queue[j];
@@ -317,13 +330,14 @@ KB_HD void evict_apply(const DevSession& S, const EvictDev& E, const uint32_t no
     if (S.proportion_present) S.q_allocated[(size_t)k * S.Q + q] = undo ? KB_DADD(S.q_allocated[(size_t)k * S.Q + q], r) : KB_DSUB(S.q_allocated[(size_t)k * S.Q + q], r);
   }
   if (S.proportion_present && undo) E.q_alloc_present[q] |= E.r_present[slot] & ~3u;
-  if (S.drf_present) update_job_share(S, j);
+  if (S.drf_present) update_job_share<RC>(S, j);
   if (S.proportion_present) update_queue_share(S, q);
   E.ctl->version += 1;
 }
 
 // Session.Pipeline / Statement.Pipeline (and Statement.unpipeline): UpdateTaskStatus(Pipelined), node.AddTask, AllocateFunc handlers
-KB_HD void pipeline_apply(const DevSession& S, const EvictDev& E, const Preemptor& P, const ClassRec& c, const uint32_t node, const bool undo) {
+template <class CR>
+KB_HD void pipeline_apply(const DevSession& S, const EvictDev& E, const Preemptor& P, const CR& c, const uint32_t node, const bool undo) {
   const uint32_t R = S.cf.R, W = S.cf.W;
   const uint32_t j = P.job, q = P.queue;
   const size_t tile_u64 = (size_t)S.ncols * TILE_NODES;
@@ -348,7 +362,7 @@ KB_HD void pipeline_apply(const DevSession& S, const EvictDev& E, const Preempto
     uint64_t& pw = t[(size_t)col_ports(R, W, w) * TILE_NODES];
     pw = undo ? (pw & ~c.port_own[w]) : (pw | c.port_own[w]);
   }
-  if (S.drf_present) update_job_share(S, j);
+  if (S.drf_present) update_job_share<CR::CAP>(S, j);
   if (S.proportion_present) update_queue_share(S, q);
   // counter path: node.AddTask puts the pod into NodeInfo.Tasks, which InterPodAffinityPriority reads for every later pod of the
   // cycle (its Spec.NodeName stays "": cachedNodeInfo.GetNodeInfo's first_unbound).  Pipelined is no AllocatedStatus: no group
@@ -377,14 +391,15 @@ KB_HD bool victim_before(const EvictDev& E, uint32_t a, uint32_t b) {
 
 // The serial part on the chosen node (thread 0): victims -> evictions until InitResreq is covered -> Pipeline.
 // stmt: log into Statement.operations (preempt) instead of recording the cache.Evict right away (reclaim).
-KB_HD void evict_commit(const DevSession& S, const EvictDev& E, const Preemptor& P, const ClassRec& c, const uint32_t node, const bool stmt) {
+template <class CR>
+KB_HD void evict_commit(const DevSession& S, const EvictDev& E, const Preemptor& P, const CR& c, const uint32_t node, const bool stmt) {
   const uint32_t R = S.cf.R, n = E.n_run;
   EvictCtl& ctl = *E.ctl;
   const uint32_t lo = E.node_off[node], hi = E.node_off[node + 1];
   const uint32_t fns = P.mode == 0 ? E.ec.reclaim_fns : E.ec.preempt_fns;
   uint32_t nv = 0, err = 0;
   for (uint32_t s = lo; s < hi; ++s) {
-    if (!evict_candidate(S, E, P, s) || !evict_is_victim(S, E, P, fns, lo, s, &err)) continue;
+    if (!evict_candidate(S, E, P, s) || !evict_is_victim<CR::CAP>(S, E, P, fns, lo, s, &err)) continue;
     if (nv == KB_EVICT_MAXV) { ctl.error = 2; return; }
     E.scratch[nv++] = s;
   }
@@ -396,11 +411,11 @@ KB_HD void evict_commit(const DevSession& S, const EvictDev& E, const Preemptor&
       while (k > 0 && victim_before(E, v, E.scratch[k - 1])) { E.scratch[k] = E.scratch[k - 1]; --k; }
       E.scratch[k] = v;
     }
-  double got[KB_MAX_R];
-  for (uint32_t k = 0; k < KB_MAX_R; ++k) got[k] = 0.0;
+  double got[CR::CAP];
+  for (uint32_t k = 0; k < CR::CAP; ++k) got[k] = 0.0;
   for (uint32_t i = 0; i < nv; ++i) {
     const uint32_t s = E.scratch[i];
-    evict_apply(S, E, node, s, false);
+    evict_apply<CR::CAP>(S, E, node, s, false);
     if (stmt) E.ops[ctl.n_ops++] = s;
     else E.evict_order[s] = ctl.n_evicted++;
     for (uint32_t k = 0; k < R; ++k) got[k] = KB_DADD(got[k], E.r_resreq[(size_t)k * n + s]);
@@ -466,9 +481,12 @@ KB_HD bool ssn_job_pipelined(const DevSession& S, const EvictDev& E, uint32_t j)
 
 // ---------------------------------------------------------------------------------------------
 // Exec policy: how the block runs the uniform control code.  X must provide
-//   tid(), nthreads(), sync(), bcast(uint32_t) (thread 0's value, with barriers), block_max(uint64_t), cls() (ClassRec& scratch
-//   every thread can read after a sync), and pre() (Preemptor& likewise).
+//   tid(), nthreads(), sync(), bcast(uint32_t) (thread 0's value, with barriers), block_max(uint64_t), cls() (ClassRecT& scratch
+//   every thread can read after a sync; its capacity is the one the class table is read in), and pre() (Preemptor& likewise).
 // ---------------------------------------------------------------------------------------------
+template <class X>
+using exec_class_t = typename std::remove_reference<decltype(std::declval<X&>().cls())>::type;
+
 struct CpuExec {
   ClassRec c; Preemptor p;
   KB_HD int tid() const { return 0; }
@@ -510,10 +528,11 @@ struct CpuExec {
 // A task an earlier allocate / backfill of this cycle Allocated on a node is a member of the groups its class joins (the
 // ClassRec.aff_own bits those placements OR into the record): its atoms' counts on that node go up by one before any eviction
 // reads them.  Only decisions from ctl.fold_step on count: an earlier evicting action of the cycle folded the ones before.
+template <uint32_t RC>
 KB_HD void evict_fold_task(const DevSession& S, const EvictDev& E, const uint32_t t) {
   const kb_decision d = S.dec[t];
   if (d.kind != KB_KIND_ALLOCATED || d.node < 0 || d.step < E.ctl->fold_step) return;     // phantom backfill tasks: no node
-  const ClassRec& c = S.classes[E.task_class[t]];
+  const ClassRecT<RC>& c = class_table<RC>(S)[E.task_class[t]];
   for (uint32_t w = 0; w < S.cf.W; ++w)
     for (uint64_t m = c.aff_own[w]; m; m &= m - 1) {
 #if defined(__CUDA_ARCH__)
@@ -526,12 +545,13 @@ KB_HD void evict_fold_task(const DevSession& S, const EvictDev& E, const uint32_
     }
 }
 
+template <uint32_t RC>
 KB_HD void evict_scan_job(const DevSession& S, const EvictDev& E, const uint32_t j) {
   int32_t w = E.job_waiting0[j];
   uint32_t first = 0xFFFFFFFFu;
   for (uint32_t i = E.pt_off[j]; i < E.pt_off[j + 1]; ++i) {
     const uint32_t t = E.pt_task[i];
-    if (E.n_atoms) evict_fold_task(S, E, t);
+    if (E.n_atoms) evict_fold_task<RC>(S, E, t);
     if (S.dec[t].kind == KB_KIND_PIPELINED) w += 1;                  // WaitingTaskNum (job_info.go:396-405)
     if (first == 0xFFFFFFFFu && task_pending(S, t)) first = i - E.pt_off[j];
   }
@@ -544,7 +564,7 @@ KB_HD void evict_init(X& x, const DevSession& S, const EvictDev& E) {
   EvictCtl& ctl = *E.ctl;
   x.sync();
   for (uint32_t j = (uint32_t)x.tid(); j < S.J && !x.jobs_scanned(); j += (uint32_t)x.nthreads()) {
-    evict_scan_job(S, E, j);
+    evict_scan_job<exec_class_t<X>::CAP>(S, E, j);
   }
   x.sync();
   if (x.tid() == 0) {
@@ -581,17 +601,18 @@ KB_HD bool evict_has_task(const DevSession& S, const EvictDev& E, uint32_t job) 
 // One preemptor against all nodes; returns `assigned` (uniform across the block).
 template <class X>
 KB_HD bool try_preemptor(X& x, const DevSession& S, const EvictDev& E, const uint32_t task, const uint32_t job, const uint32_t mode, const bool stmt) {
+  constexpr uint32_t RC = exec_class_t<X>::CAP;
   EvictCtl& ctl = *E.ctl;
   x.sync();
   if (x.tid() == 0) {
     Preemptor& P = x.pre();
     P.task = task; P.job = job; P.queue = S.job_queue[job]; P.cls = E.task_class[task]; P.mode = mode;
-    if (!ctl.cls_valid || ctl.cls_id != P.cls) { x.cls() = S.classes[P.cls]; ctl.cls_id = P.cls; ctl.cls_valid = 1; }      // 408 B: only when it changes
+    if (!ctl.cls_valid || ctl.cls_id != P.cls) { x.cls() = class_table<RC>(S)[P.cls]; ctl.cls_id = P.cls; ctl.cls_valid = 1; }      // 408 B: only when it changes
     P.ls = 0.0;
     if (mode != 0 && (E.ec.preempt_fns & EVF_DRF)) {
-      double la[KB_MAX_R];
+      double la[RC];
       for (uint32_t k = 0; k < S.cf.R; ++k) la[k] = KB_DADD(S.job_alloc[(size_t)k * S.J + job], x.cls().resreq[k]);
-      P.ls = drf_share_of(S, la);
+      P.ls = drf_share_of<RC>(S, la);
     }
     ctl.tasks_processed += 1;
     ctl.pairs_logical += (unsigned long long)S.N;
@@ -599,7 +620,7 @@ KB_HD bool try_preemptor(X& x, const DevSession& S, const EvictDev& E, const uin
   }
   x.sync();
   const Preemptor& P = x.pre();
-  const ClassRec& c = x.cls();
+  const exec_class_t<X>& c = x.cls();
   // An identical sweep (same class, same filter, nothing changed since) that found no node finds none again: skip it.  This holds
   // with preferred node-affinity terms and inter-pod weights too: their scores only order the valid nodes, whether a valid node exists
   // does not depend on them (and a Pipeline, which moves the kind counts, bumps ctl.version).
@@ -689,12 +710,12 @@ KB_HD void run_preempt(X& x, const DevSession& S, const EvictDev& E) {
             if (op & 0x80000000u) {
               const uint32_t t = op & 0x7FFFFFFFu;
               Preemptor P; P.task = t; P.job = pj; P.queue = S.job_queue[pj]; P.cls = E.task_class[t]; P.mode = 1; P.ls = 0;
-              pipeline_apply(S, E, P, S.classes[P.cls], (uint32_t)S.dec[t].node, true);
+              pipeline_apply(S, E, P, class_table<exec_class_t<X>::CAP>(S)[P.cls], (uint32_t)S.dec[t].node, true);
             } else {
               // the slot's node: binary search in node_off
               uint32_t lo = 0, hi = S.N;
               while (hi - lo > 1) { const uint32_t mid = (lo + hi) / 2; if (E.node_off[mid] <= op) lo = mid; else hi = mid; }
-              evict_apply(S, E, lo, op, true);
+              evict_apply<exec_class_t<X>::CAP>(S, E, lo, op, true);
             }
           }
           if (S.aff.on) *S.aff.first_unbound = ctl.stmt_fu;     // the Statement's evictions never move it, its Pipelines only lower it

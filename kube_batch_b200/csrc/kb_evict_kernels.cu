@@ -58,7 +58,9 @@ __device__ __forceinline__ long long ev_warp_min(const long long v) {
   return (long long)(((unsigned long long)(unsigned)mhi << 32) | mlo);
 }
 
-// the master thread's Exec: single-threaded control, the sweep is farmed out
+// the master thread's Exec: single-threaded control, the sweep is farmed out.  RC: class capacity of the session (ClassRecT), the
+// capacity of the mailbox record (EvictCtl.cls / cls_wide) and of the workers' copy
+template <uint32_t RC>
 struct MasterExec {
   EvictCtl* g;
   uint32_t seq;
@@ -68,7 +70,10 @@ struct MasterExec {
   __device__ __forceinline__ uint32_t bcast(uint32_t v) { return v; }
   __device__ __forceinline__ bool jobs_scanned() const { return true; }      // evict_scan_kernel ran before this kernel
   __device__ __forceinline__ void clear_max() {}
-  __device__ __forceinline__ ClassRec& cls() { return g->cls; }
+  __device__ __forceinline__ ClassRecT<RC>& cls() {
+    if constexpr (RC == KB_CLASS_R) return g->cls;
+    else return g->cls_wide;
+  }
   __device__ __forceinline__ Preemptor& pre() { return g->pre; }
   __device__ __forceinline__ void post(const uint32_t pass) {     // one command to every worker CTA, back when all have arrived
     g->pass = pass;
@@ -79,7 +84,7 @@ struct MasterExec {
     const uint32_t nw = g->n_workers;
     while (ev_ld_acquire(&g->arrived) < nw) __nanosleep(40);
   }
-  __device__ __forceinline__ uint64_t sweep(const DevSession& S, const EvictDev&, const Preemptor& P, const ClassRec&) {
+  __device__ __forceinline__ uint64_t sweep(const DevSession& S, const EvictDev&, const Preemptor& P, const ClassRecT<RC>&) {
     // preferred node-affinity terms: pass 1 leaves the max count in g->pmax, which is then the sweep's normalisation.  It is
     // taken afresh for every sweep: a Pipeline raises a node's pod count, and max_pods can drop that node together with its count.
     // inter-pod weight list: clear dom_sum, fill it, reduce min / max (and pmax in the same pass) — three commands.
@@ -91,14 +96,14 @@ struct MasterExec {
   }
 };
 
-template <int PREEMPT>
+template <int PREEMPT, uint32_t RC = KB_NARROW_R>
 __global__ void __launch_bounds__(EVICT_THREADS, 1)
 evict_kernel(const __grid_constant__ DevSession S, const __grid_constant__ EvictDev E) {
   EvictCtl* g = E.ctl;
   if (blockIdx.x == gridDim.x - 1) {
     // ---------------- master ----------------
     if (threadIdx.x != 0) return;
-    MasterExec x{g, 0u};
+    MasterExec<RC> x{g, 0u};
     if (PREEMPT) run_preempt(x, S, E);
     else run_reclaim(x, S, E);
     __threadfence();
@@ -106,7 +111,7 @@ evict_kernel(const __grid_constant__ DevSession S, const __grid_constant__ Evict
     return;
   }
   // ---------------- workers ----------------
-  __shared__ ClassRec s_cls;
+  __shared__ ClassRecT<RC> s_cls;
   __shared__ Preemptor s_pre;
   __shared__ ClassPref s_pref;                     // preferred node-affinity terms of class s_pref_cls
   __shared__ ClassAff s_aff;                       // inter-pod weight list record of class s_aff_cls
@@ -134,7 +139,7 @@ evict_kernel(const __grid_constant__ DevSession S, const __grid_constant__ Evict
     {
       const uint32_t* src = reinterpret_cast<const uint32_t*>(&g->cls);
       uint32_t* dst = reinterpret_cast<uint32_t*>(&s_cls);
-      for (uint32_t i = threadIdx.x; i < sizeof(ClassRec) / 4; i += EVICT_THREADS) dst[i] = src[i];
+      for (uint32_t i = threadIdx.x; i < sizeof(ClassRecT<RC>) / 4; i += EVICT_THREADS) dst[i] = src[i];
       const uint32_t* ps = reinterpret_cast<const uint32_t*>(&g->pre);
       uint32_t* pd = reinterpret_cast<uint32_t*>(&s_pre);
       for (uint32_t i = threadIdx.x; i < sizeof(Preemptor) / 4; i += EVICT_THREADS) pd[i] = ps[i];
@@ -261,9 +266,10 @@ evict_kernel(const __grid_constant__ DevSession S, const __grid_constant__ Evict
 }
 
 // evict_init's per-job scan (WaitingTaskNum, first Pending task, the job's Allocated members into the atom counts), one thread per job
+template <uint32_t RC = KB_NARROW_R>
 __global__ void evict_scan_kernel(const __grid_constant__ DevSession S, const __grid_constant__ EvictDev E) {
   const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
-  if (j < S.J) evict_scan_job(S, E, j);
+  if (j < S.J) evict_scan_job<RC>(S, E, j);
 }
 
 cudaError_t launch_evict(const bool preempt, const DevSession& S, const EvictDev& E, const int sm_count, cudaStream_t stream) {
@@ -277,10 +283,16 @@ cudaError_t launch_evict(const bool preempt, const DevSession& S, const EvictDev
   if (c != cudaSuccess) return c;
   c = cudaMemsetAsync(reinterpret_cast<char*>(E.ctl) + offsetof(EvictCtl, cls_valid), 0, 4, stream);
   if (c != cudaSuccess) return c;
-  if (S.J) evict_scan_kernel<<<(S.J + 255) / 256, 256, 0, stream>>>(S, E);
+  // a session with more resource dimensions than the narrow class record holds runs the wide instances (kb_build.h)
+  const bool wide = S.cf.R > KB_NARROW_R;
+  if (S.J) {
+    if (wide) evict_scan_kernel<KB_MAX_R><<<(S.J + 255) / 256, 256, 0, stream>>>(S, E);
+    else evict_scan_kernel<><<<(S.J + 255) / 256, 256, 0, stream>>>(S, E);
+  }
   DevSession s = S; EvictDev ev = E;
   void* args[] = {(void*)&s, (void*)&ev};
-  const void* fn = preempt ? (const void*)evict_kernel<1> : (const void*)evict_kernel<0>;
+  const void* fn = wide ? (preempt ? (const void*)evict_kernel<1, KB_MAX_R> : (const void*)evict_kernel<0, KB_MAX_R>)
+                        : (preempt ? (const void*)evict_kernel<1> : (const void*)evict_kernel<0>);
   return cudaLaunchCooperativeKernel(fn, dim3(workers + 1), dim3(EVICT_THREADS), args, 0, stream);
 }
 

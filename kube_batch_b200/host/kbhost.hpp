@@ -611,7 +611,7 @@ inline Flat Flatten(const framework::Session& ssn) {
   for (auto& jk : ssn.Jobs) for (auto& tk : jk.second->Tasks) { for (auto& s : tk.second->Resreq.ScalarResources) sc.insert(s.first); for (auto& s : tk.second->InitResreq.ScalarResources) sc.insert(s.first); }
   f.dims = {"cpu", "memory"}; for (auto& s : sc) f.dims.push_back(s);
   f.R = (uint32_t)f.dims.size();
-  if (f.R > KB_MAX_R) throw std::runtime_error("too many scalar resources for KB_MAX_R");
+  if (f.R > KB_MAX_R) throw Unsupported(std::to_string(f.R) + " resource dimensions > KB_MAX_R (" + std::to_string(KB_MAX_R) + ")");
   std::vector<std::shared_ptr<api::NodeInfo>> nodes; for (auto& kv : ssn.Nodes) nodes.push_back(kv.second);       // std::map: ascending Name
   std::vector<std::shared_ptr<api::QueueInfo>> queues; for (auto& kv : ssn.Queues) queues.push_back(kv.second);
   std::vector<std::shared_ptr<api::JobInfo>> jobs; for (auto& kv : ssn.Jobs) jobs.push_back(kv.second);          // ascending JobID
