@@ -69,7 +69,9 @@ type Flat struct {
 
 const (
 	maxR         = 32 // KB_MAX_R
-	maxW         = 4  // KB_MAX_W
+	maxW         = 16 // KB_MAX_W
+	narrowR      = 8  // KB_NARROW_R (kb_core.h): sessions with more dimensions take at most narrowW words
+	narrowW      = 4  // KB_NARROW_W
 	maxAffTerms  = 4  // KB_MAX_AFF_TERMS
 	maxPrefTerms = 4  // KB_MAX_PREF_TERMS
 )
@@ -429,7 +431,10 @@ func Flatten(ssn *framework.Session) (*Flat, error) {
 	}
 	W := (max1(need) + 63) / 64
 	if W > maxW {
-		return nil, &ErrUnsupported{fmt.Sprintf("%d label / taint / port atoms > 64 x KB_MAX_W", need)}
+		return nil, &ErrUnsupported{fmt.Sprintf("%d label / taint / port atoms > 64 x KB_MAX_W (%d)", need, maxW)}
+	}
+	if R > narrowR && W > narrowW {
+		return nil, &ErrUnsupported{fmt.Sprintf("%d resource dimensions > KB_NARROW_R (%d) with %d atoms > 64 x KB_NARROW_W (%d)", R, narrowR, need, narrowW)}
 	}
 	f.R, f.W, f.N, f.T, f.J, f.Q = uint32(R), uint32(W), uint32(N), uint32(T), uint32(J), uint32(Q)
 

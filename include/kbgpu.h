@@ -30,7 +30,7 @@ extern "C" {
 
 /* Compile-time capacity of the dense encodings. */
 #define KB_MAX_R 32         /* resource dims: 0 = cpu (milli), 1 = memory (bytes), 2.. = scalar resources (milli); one bit per dim in the *_present masks */
-#define KB_MAX_W 4          /* 64-bit words per label / taint / host-port bitmask */
+#define KB_MAX_W 16         /* 64-bit words per label / taint / host-port bitmask (1024 atoms per family) */
 #define KB_MAX_PREF_TERMS 4   /* preferred node-affinity terms per task */
 #define KB_MAX_AFF_TERMS 4  /* OR-ed required node-affinity terms carried per task */
 #define KB_MAX_Q 65536      /* queues (kb_session_load refuses more with KB_E_BADARG) */
@@ -167,7 +167,8 @@ typedef struct kb_snapshot {
   uint32_t abi_version;     /* KB_ABI_VERSION */
   uint32_t R;               /* 2..KB_MAX_R (> KB_MAX_R: KB_E_BADARG).  R <= 8 runs the 8-dimension kernel instances, 9..32 the
                                32-dimension ones (wider class records and node tiles); R > 8 with KB_ENGINE_SHARD: KB_E_UNSUPPORTED_FEATURE */
-  uint32_t W;               /* 1..KB_MAX_W */
+  uint32_t W;               /* 1..KB_MAX_W (> KB_MAX_W: KB_E_BADARG).  W <= 4 runs the 4-word kernel instances, 5..16 the wide-atom
+                               ones; W > 4 with R > 8 or with KB_ENGINE_SHARD: KB_E_UNSUPPORTED_FEATURE */
   uint32_t N, T, J, Q;
   uint32_t flags;           /* KB_SNAPSHOT_* */
 

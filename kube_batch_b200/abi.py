@@ -16,7 +16,10 @@ KB_ENGINE_NO_PIPE = 1 << 5
 KB_ENGINE_SHARD = 1 << 6
 KB_ABI_VERSION = 3
 KB_MAX_R = 32
-KB_MAX_W = 4
+KB_MAX_W = 16
+# kb_core.h: sessions above either narrow capacity run the wide (R) or wide-atom (W) kernel instances, never both
+KB_NARROW_R = 8
+KB_NARROW_W = 4
 KB_MAX_AFF_TERMS = 4
 KB_MAX_PREF_TERMS = 4
 KB_MAX_Q = 65536

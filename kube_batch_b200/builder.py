@@ -320,7 +320,9 @@ class SessionBuilder:
                     port_atoms[sp] = len(port_atoms)
         need = max(len(req_atoms), len(taint_atoms), len(port_atoms), 1)
         W = max(W, (need + 63) // 64)
-        assert W <= abi.KB_MAX_W, "too many atoms for KB_MAX_W words"
+        assert W <= abi.KB_MAX_W, f"{need} label / taint / port atoms > 64 x KB_MAX_W ({abi.KB_MAX_W})"
+        assert R <= abi.KB_NARROW_R or W <= abi.KB_NARROW_W, \
+            f"{R} resource dimensions > KB_NARROW_R ({abi.KB_NARROW_R}) with {need} atoms > 64 x KB_NARROW_W ({abi.KB_NARROW_W})"
 
         s = Snapshot(R, W, len(nodes), len(pending), len(groups), len(queues))
 

@@ -12,6 +12,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <string>
+#include <type_traits>
 #include <unordered_map>
 #include <map>
 #include <vector>
@@ -323,10 +324,11 @@ inline bool allow_pref_legacy(bool allow_pref, uint32_t world) { return allow_pr
 
 // Tiles per scan iteration of the per-visit kernels: up to 4 (16 warps), bounded by the shared memory left for the two staging
 // buffers next to VisitSmem — ~190 KB next to the narrow instances' ~26 KB, ~160 KB next to the wide instances' ~51 KB (class
-// record and candidate slots of up to 82 columns).  The widest record (R = 32, W = 4: 82 columns, 84 KB per tile) gets tpi = 1.
+// record and candidate slots of up to 82 columns) and the wide-atom instances' (up to 70 columns).  The widest records (R = 32,
+// W = 4: 82 columns, 84 KB per tile; R = 8, W = 16: 70 columns, 72 KB per tile) get tpi = 1.
 inline uint32_t scan_tpi(const uint32_t R, const uint32_t W) {
   const size_t tile_bytes = (size_t)tile_ncols(R, W) * TILE_NODES * 8;
-  const size_t budget = (R > KB_NARROW_R ? 160 : 190) * 1024;
+  const size_t budget = (R > KB_NARROW_R || W > KB_NARROW_W ? 160 : 190) * 1024;
   uint32_t tpi = 4;
   while (tpi > 1 && 2 * tpi * tile_bytes > budget) --tpi;
   return tpi;
@@ -338,8 +340,9 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
                          uint32_t kchain = 1 /* classes per launch: 1, 2 or 4 (single GPU, no overlap) */,
                          bool allow_pref = false /* accept preferred node-affinity terms (tests/emu prototype only) */,
                          int pipe_mode = 0 /* persistent pipeline (cycle_kernel): 0 off, 1 when the geometry allows it */,
-                         bool wide_classes = false /* the caller reads class tables of capacity KB_MAX_R (class_table<KB_MAX_R>):
-                                                      sessions with R > KB_CLASS_R are accepted (the engine's wide kernel instances) */) {
+                         bool wide_classes = false /* the caller reads class tables of ClassRecWide / ClassRecAtoms (class_table<CR>):
+                                                      sessions with R > KB_CLASS_R or W > KB_CLASS_W are accepted (the engine's wide and
+                                                      wide-atom kernel instances) */) {
   if (!s) return bfail(e, KB_E_BADARG, "snapshot is NULL");
   if (s->abi_version != KB_ABI_VERSION) return bfail(e, KB_E_BADARG, "snapshot abi_version %u != %u", s->abi_version, KB_ABI_VERSION);
   const kb_pod_affinity* pa = s->pod_affinity;
@@ -352,12 +355,22 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
   if (s->flags & ~(KB_SNAPSHOT_PLACED_POD_AFFINITY | KB_SNAPSHOT_LISTED_POD_WITHOUT_NODE)) return bfail(e, KB_E_BADARG, "unknown kb_snapshot.flags bits 0x%x", s->flags);
   if (s->R < 2 || s->R > KB_MAX_R || s->W < 1 || s->W > KB_MAX_W)
     return bfail(e, KB_E_BADARG, "R=%u / W=%u out of range (2 <= R <= KB_MAX_R = %u, 1 <= W <= KB_MAX_W = %u)", s->R, s->W, (unsigned)KB_MAX_R, (unsigned)KB_MAX_W);
+  // no record holds both: the widest node tile (R = 32, W = 16: 118 columns) would not fit next to the wide VisitSmem staging
+  if (s->R > KB_NARROW_R && s->W > KB_NARROW_W)
+    return bfail(e, KB_E_UNSUPPORTED_FEATURE, "R=%u resource dimensions with W=%u mask words: sessions with R > KB_NARROW_R (%u) take at most "
+                 "KB_NARROW_W (%u) words, sessions with W > KB_NARROW_W at most KB_NARROW_R dimensions", s->R, s->W, (unsigned)KB_NARROW_R,
+                 (unsigned)KB_NARROW_W);
   if (s->R > KB_CLASS_R && !wide_classes)
     return bfail(e, KB_E_BADARG, "R=%u: this build reads class records of %u resource dimensions (ClassRec)", s->R, (unsigned)KB_CLASS_R);
-  // the sharded exchange carries node records of at most KB_NARROW_R dimensions (P2P_RANK_U64)
+  if (s->W > KB_CLASS_W && !wide_classes)
+    return bfail(e, KB_E_BADARG, "W=%u: this build reads class records of %u mask words (ClassRec)", s->W, (unsigned)KB_CLASS_W);
+  // the sharded exchange carries node records of at most KB_NARROW_R dimensions and KB_NARROW_W words (P2P_RANK_U64)
   if (world > 1 && s->R > KB_NARROW_R)
     return bfail(e, KB_E_UNSUPPORTED_FEATURE, "R=%u resource dimensions with a sharded node axis (KB_ENGINE_SHARD): the exchange carries node records "
                  "of at most %u dimensions", s->R, (unsigned)KB_NARROW_R);
+  if (world > 1 && s->W > KB_NARROW_W)
+    return bfail(e, KB_E_UNSUPPORTED_FEATURE, "W=%u mask words with a sharded node axis (KB_ENGINE_SHARD): the exchange carries node records "
+                 "of at most KB_NARROW_W (%u) words", s->W, (unsigned)KB_NARROW_W);
   if (s->Q > KB_MAX_Q) return bfail(e, KB_E_BADARG, "Q=%u > KB_MAX_Q (%u)", s->Q, (unsigned)KB_MAX_Q);
   if (s->N >= 0xFFFFFFF0u) return bfail(e, KB_E_BADARG, "N too large for the packed key");
   const uint32_t R = s->R, W = s->W, N = s->N, T = s->T, J = s->J, Q = s->Q;
@@ -535,7 +548,9 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
       if (s->node_idle[(size_t)r * N + n] <= -eps)
         return bfail(e, KB_E_BADARG, "node %u: Idle is negative in dim %u (over-committed node: the reference cache would not produce it)", n, r);
     }
-  std::vector<ClassRec> classes;
+  // the class identity: every dimension ClassRec holds and every mask word the session has; written to the class table in the
+  // session's record type (write_classes)
+  std::vector<ClassRecBuild> classes;
   // dims KB_CLASS_R..R-1 of every class (initreq, then resreq; empty when R <= KB_CLASS_R): part of the class identity, joined
   // with `classes` into the wide records of the class table
   const uint32_t RH = R > KB_CLASS_R ? R - KB_CLASS_R : 0u;
@@ -543,10 +558,10 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
   std::vector<double> hi(2 * (size_t)RH, 0.0);
   auto init_of = [&](uint32_t id, uint32_t k) { return k < KB_CLASS_R ? classes[id].initreq[k] : class_hi[(size_t)id * 2 * RH + (k - KB_CLASS_R)]; };
   auto same_hi = [&](uint32_t id) { return RH == 0 || memcmp(&class_hi[(size_t)id * 2 * RH], hi.data(), 2 * (size_t)RH * 8) == 0; };
-  std::vector<ClassPref>& class_pref = B.class_pref;
-  class_pref.clear(); B.has_pref = false;
+  std::vector<ClassPrefBuild> class_pref;
+  B.class_pref.clear(); B.has_pref = false;
   auto pref_of = [&](uint32_t t) {
-    ClassPref cp;
+    ClassPrefBuild cp;
     memset(&cp, 0, sizeof cp);
     if (!(s->task_flags[t] & KB_TASK_HAS_PREFERRED_NODE_AFFINITY)) return cp;
     if (!s->task_n_pref_terms || !s->task_pref_terms || !s->task_pref_weights) { cp.n = 0xFFFFFFFFu; return cp; }   // reported by the caller
@@ -631,17 +646,48 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
   std::vector<uint32_t> task_class(T, 0);
   std::vector<uint8_t> task_empty(T, 0);
   {
-    // open-addressing table keyed by a 64-bit hash of the record, verified with memcmp; a task usually equals its
-    // predecessor (PodGroups are homogeneous), so that case is checked first
+    // open-addressing table keyed by a 64-bit hash of the record, verified field by field; a task usually equals its
+    // predecessor (PodGroups are homogeneous), so that case is checked first.  Records and preferred terms are read through
+    // their first W mask words only (the rest are 0), so a narrow session hashes and compares no more than its ClassRec.
     std::vector<uint32_t> table(1024, 0xFFFFFFFFu);
     std::vector<uint64_t> class_hash;
-    auto hash_rec = [](const ClassRec& c) {
-      const uint64_t* w = reinterpret_cast<const uint64_t*>(&c);
+    auto rec_words = [W](const ClassRecBuild& c, auto&& fn) {
+      for (uint32_t k = 0; k < KB_CLASS_R; ++k) { uint64_t a, b; memcpy(&a, &c.initreq[k], 8); memcpy(&b, &c.resreq[k], 8); fn(a); fn(b); }
+      fn((uint64_t)c.nz_cpu); fn((uint64_t)c.nz_mem);
+      for (uint32_t w = 0; w < W; ++w) {
+        fn(c.sel_req[w]); fn(c.tol[w]); fn(c.port_own[w]); fn(c.port_conflict[w]); fn(c.aff_own[w]);
+        for (uint32_t a = 0; a < KB_MAX_AFF_TERMS; ++a) fn(c.aff[a][w]);
+      }
+      fn(((uint64_t)c.n_aff << 32) | c.flags);
+    };
+    auto pref_words = [W](const ClassPrefBuild& p, auto&& fn) {
+      for (uint32_t k = 0; k < KB_MAX_PREF_TERMS; ++k) {
+        for (uint32_t w = 0; w < W; ++w) fn(p.term[k][w]);
+        fn((uint64_t)(uint32_t)p.weight[k]);
+      }
+      fn(p.n);
+    };
+    auto hash_rec = [&](const ClassRecBuild& c) {
       uint64_t h = 0x9E3779B97F4A7C15ull;
-      for (size_t i = 0; i < sizeof(ClassRec) / 8; ++i) { h ^= w[i] + 0x9E3779B97F4A7C15ull + (h << 6) + (h >> 2); h *= 0xFF51AFD7ED558CCDull; h ^= h >> 32; }
+      rec_words(c, [&](uint64_t x) { h ^= x + 0x9E3779B97F4A7C15ull + (h << 6) + (h >> 2); h *= 0xFF51AFD7ED558CCDull; h ^= h >> 32; });
       return h;
     };
-    static_assert(sizeof(ClassRec) % 8 == 0, "ClassRec is hashed as 64-bit words");
+    auto same_rec = [&](const ClassRecBuild& a, const ClassRecBuild& b) {
+      uint64_t va[KB_CLASS_R * 2 + 3 + 9 * KB_MAX_W];
+      size_t n = 0, i = 0;
+      bool same = true;
+      rec_words(a, [&](uint64_t x) { va[n++] = x; });
+      rec_words(b, [&](uint64_t x) { same = same && va[i++] == x; });
+      return same;
+    };
+    auto same_pref = [&](const ClassPrefBuild& a, const ClassPrefBuild& b) {
+      uint64_t va[KB_MAX_PREF_TERMS * (KB_MAX_W + 1) + 1];
+      size_t n = 0, i = 0;
+      bool same = true;
+      pref_words(a, [&](uint64_t x) { va[n++] = x; });
+      pref_words(b, [&](uint64_t x) { same = same && va[i++] == x; });
+      return same;
+    };
     uint32_t prev_class = 0xFFFFFFFFu;
     // PodGroups are homogeneous: most tasks carry exactly the fields of their predecessor.  Comparing the flattened columns of
     // t and t-1 (bit patterns, like the memcmp of the records below) is far cheaper than building and hashing a record.
@@ -653,8 +699,7 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
       if (s->task_flags[t] != s->task_flags[t - 1] || s->task_n_aff_terms[t] != s->task_n_aff_terms[t - 1] ||
           s->task_nz_cpu[t] != s->task_nz_cpu[t - 1] || s->task_nz_mem[t] != s->task_nz_mem[t - 1]) return false;
       if (s->task_flags[t] & KB_TASK_HAS_PREFERRED_NODE_AFFINITY) {
-        const ClassPref a = pref_of(t), b = pref_of(t - 1);
-        if (memcmp(&a, &b, sizeof a) != 0) return false;
+        if (!same_pref(pref_of(t), pref_of(t - 1))) return false;
       }
       for (uint32_t r = 0; r < R; ++r) {
         const size_t i = (size_t)r * T + t;
@@ -672,6 +717,8 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
       }
       return true;
     };
+    ClassRecBuild rec;                    // the record of the task at hand, reused: clearing 1.3 KB per task would cost more than the rest
+    memset(&rec, 0, sizeof rec);
     for (uint32_t t = 0; t < T; ++t) {
       if (t > 0 && prev_class != 0xFFFFFFFFu && same_as_prev(t)) {     // t-1 passed every check below with the same values
         task_class[t] = prev_class; task_empty[t] = task_empty[t - 1];
@@ -681,14 +728,13 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
         return bfail(e, KB_E_UNSUPPORTED_FEATURE, "task %u carries inter-pod affinity terms but the snapshot has no kb_pod_affinity (no CPU fallback)", t);
       if ((s->task_flags[t] & KB_TASK_HAS_PREFERRED_NODE_AFFINITY) && !pa && !will_pipe && !pref_legacy)
         return bfail(e, KB_E_UNSUPPORTED_FEATURE, "task %u carries preferred node-affinity terms: neither the persistent pipeline nor the counter path is available", t);
-      ClassPref cp = pref_of(t);
+      ClassPrefBuild cp = pref_of(t);
       if (cp.n) {
         if (cp.n > KB_MAX_PREF_TERMS) return bfail(e, KB_E_BADARG, "task %u: preferred node-affinity arrays missing or n_pref_terms > KB_MAX_PREF_TERMS", t);
         B.has_pref = true;
       }
       if (s->task_n_aff_terms[t] > KB_MAX_AFF_TERMS) return bfail(e, KB_E_BADARG, "task %u: n_aff_terms > KB_MAX_AFF_TERMS", t);
-      ClassRec c;
-      memset(&c, 0, sizeof c);
+      ClassRecBuild& c = rec;             // every field a task sets is set below; words >= W and dims >= R stay 0
       for (uint32_t r = 0; r < R; ++r) {
         const double ir = s->task_initreq[(size_t)r * T + t], rr = s->task_resreq[(size_t)r * T + t];
         if (r < KB_CLASS_R) { c.initreq[r] = ir; c.resreq[r] = rr; }
@@ -703,24 +749,25 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
         c.tol[w] = s->task_tol[(size_t)w * T + t];
         c.port_own[w] = s->task_port_own[(size_t)w * T + t];
         c.port_conflict[w] = s->task_port_conflict[(size_t)w * T + t];
-        for (uint32_t a = 0; a < c.n_aff; ++a) c.aff[a][w] = s->task_aff_terms[((size_t)a * W + w) * T + t];
+        c.aff_own[w] = 0;
+        for (uint32_t a = 0; a < KB_MAX_AFF_TERMS; ++a) c.aff[a][w] = a < c.n_aff ? s->task_aff_terms[((size_t)a * W + w) * T + t] : 0ull;
       }
       if (aff_as_atoms) {                 // host-level anti-affinity as atoms: forbidden groups conflict, joined groups are set by Allocate
         if (hc.cf.predicates) atoms_of(pa_full->task_forbid[t], t, KB_XGROUP_FORBID, c.port_conflict);
         atoms_of(pa_full->task_contrib[t], t, KB_XGROUP_CONTRIB, c.aff_own);
       }
       task_empty[t] = res_is_empty(R, [&](uint32_t k) { return k < KB_CLASS_R ? c.resreq[k] : hi[RH + k - KB_CLASS_R]; }) ? 1 : 0;   // allocate.go:113-118
-      if (prev_class != 0xFFFFFFFFu && memcmp(&classes[prev_class], &c, sizeof c) == 0 && memcmp(&class_pref[prev_class], &cp, sizeof cp) == 0 &&
+      if (prev_class != 0xFFFFFFFFu && same_rec(classes[prev_class], c) && same_pref(class_pref[prev_class], cp) &&
           same_hi(prev_class)) {
         task_class[t] = prev_class; continue; }
       uint64_t h = hash_rec(c);
-      if (cp.n) { const uint64_t* w = reinterpret_cast<const uint64_t*>(&cp); for (size_t i = 0; i < sizeof(ClassPref) / 8; ++i) h = (h ^ w[i]) * 0xFF51AFD7ED558CCDull + (h >> 29); }
+      if (cp.n) pref_words(cp, [&](uint64_t x) { h = (h ^ x) * 0xFF51AFD7ED558CCDull + (h >> 29); });
       for (uint32_t i = 0; i < 2 * RH; ++i) { uint64_t u; memcpy(&u, &hi[i], 8); h = (h ^ u) * 0xFF51AFD7ED558CCDull + (h >> 29); }
       size_t mask = table.size() - 1, slot = (size_t)h & mask;
       uint32_t found = 0xFFFFFFFFu;
       while (table[slot] != 0xFFFFFFFFu) {
         const uint32_t id = table[slot];
-        if (class_hash[id] == h && memcmp(&classes[id], &c, sizeof c) == 0 && memcmp(&class_pref[id], &cp, sizeof cp) == 0 && same_hi(id)) { found = id; break; }
+        if (class_hash[id] == h && same_rec(classes[id], c) && same_pref(class_pref[id], cp) && same_hi(id)) { found = id; break; }
         slot = (slot + 1) & mask;
       }
       if (found == 0xFFFFFFFFu) {
@@ -740,10 +787,14 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
     }
   }
   if (classes.empty()) {
-    ClassRec c; memset(&c, 0, sizeof c); classes.push_back(c); ClassPref cp; memset(&cp, 0, sizeof cp); class_pref.push_back(cp);
+    ClassRecBuild c; memset(&c, 0, sizeof c); classes.push_back(c); ClassPrefBuild cp; memset(&cp, 0, sizeof cp); class_pref.push_back(cp);
     class_hi.assign(2 * (size_t)RH, 0.0);
   }
-  static_assert(sizeof(ClassPref) % 8 == 0, "ClassPref is hashed as 64-bit words");
+  // the host copy tests/emu reads, in ClassRec's word capacity (a session with more words runs on the device only)
+  if (W <= KB_CLASS_W) {
+    B.class_pref.resize(class_pref.size());
+    for (size_t k = 0; k < class_pref.size(); ++k) pref_copy(B.class_pref[k], class_pref[k]);
+  }
   if (B.has_pref) hc.cf.score_bias += 10ll * (hc.w_nodeaff < 0 ? -(int64_t)hc.w_nodeaff : 0);
   const uint32_t C = (uint32_t)classes.size();
   B.aff = AffDev{};
@@ -864,7 +915,10 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
   om.recvbuf = mut.alloc((size_t)std::max(1u, world) * xchg_u64(ncols) * 8);
   om.bf_job_pos = mut.alloc((size_t)std::max(1u, J) * 4);
   om.bf_ctl = mut.alloc(sizeof(Ctl));
-  const size_t class_bytes = RH ? sizeof(ClassRecWide) : sizeof(ClassRec);
+  // the session's record type: ClassRecWide for R > KB_CLASS_R, ClassRecAtoms for W > KB_CLASS_W, else ClassRec
+  const bool atoms = W > KB_CLASS_W;
+  const size_t class_bytes = RH ? sizeof(ClassRecWide) : atoms ? sizeof(ClassRecAtoms) : sizeof(ClassRec);
+  const size_t pref_bytes = atoms ? sizeof(ClassPrefT<KB_MAX_W>) : sizeof(ClassPref);
   oi.classes = imm.alloc((size_t)C * class_bytes);
   oi.total_hi = imm.alloc((size_t)std::max(1u, RH) * 8);
   oi.ord_task = imm.alloc((size_t)std::max(1u, To) * 4);
@@ -892,7 +946,7 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
   oi.bf_jobs_off = imm.alloc(2 * 4);
   oi.bf_classes = imm.alloc((size_t)(Tb ? C : 1) * class_bytes);
   oi.ord_chain = imm.alloc((size_t)std::max(1u, To) * (KB_CHAIN_MAX - 1) * 4);
-  oi.class_pref = imm.alloc((size_t)(B.has_pref ? C : 1) * sizeof(ClassPref));
+  oi.class_pref = imm.alloc((size_t)(B.has_pref ? C : 1) * pref_bytes);
   if (pa) {
     oi.aff_node_domain = imm.alloc((size_t)std::max(1u, pa->n_keysets) * std::max(1u, N) * 4);
     oi.aff_keyset_off = imm.alloc((size_t)(pa->n_keysets + 1) * 4);
@@ -954,28 +1008,33 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
   }
 
   // ---------------- immutable job / queue / class tables ----------------
-  // the class table in the session's capacity; a wide record joins the narrow part with its dims past KB_CLASS_R
-  auto write_classes = [&](unsigned char* dst, const bool backfill) {
+  // the class table in the session's record type; a wide record joins the narrow part with its dims past KB_CLASS_R
+  auto write_as = [&](auto* tab, const bool backfill) {
+    using CR = typename std::remove_pointer<decltype(tab)>::type;
     for (uint32_t k = 0; k < C; ++k) {
-      if (!RH) {
-        ClassRec& d = reinterpret_cast<ClassRec*>(dst)[k];
-        d = classes[k];
-        if (backfill) for (uint32_t r = 0; r < KB_CLASS_R; ++r) d.initreq[r] = d.resreq[r];
-        continue;
-      }
-      ClassRecWide w;
+      CR w;
       memset(&w, 0, sizeof w);
       class_copy(w, classes[k]);
-      for (uint32_t r = KB_CLASS_R; r < R; ++r) {
+      for (uint32_t r = KB_CLASS_R; r < R && r < CR::CAP; ++r) {
         w.initreq[r] = class_hi[(size_t)k * 2 * RH + (r - KB_CLASS_R)];
         w.resreq[r] = class_hi[(size_t)k * 2 * RH + RH + (r - KB_CLASS_R)];
       }
-      if (backfill) for (uint32_t r = 0; r < KB_MAX_R; ++r) w.initreq[r] = w.resreq[r];
-      memcpy(dst + (size_t)k * sizeof(ClassRecWide), &w, sizeof w);
+      if (backfill) for (uint32_t r = 0; r < CR::CAP; ++r) w.initreq[r] = w.resreq[r];
+      memcpy(&tab[k], &w, sizeof w);
     }
   };
+  auto write_classes = [&](unsigned char* dst, const bool backfill) {
+    if (RH) write_as(reinterpret_cast<ClassRecWide*>(dst), backfill);
+    else if (atoms) write_as(reinterpret_cast<ClassRecAtoms*>(dst), backfill);
+    else write_as(reinterpret_cast<ClassRec*>(dst), backfill);
+  };
   write_classes(imm.host.data() + oi.classes, false);
-  if (B.has_pref) memcpy(imm.host.data() + oi.class_pref, class_pref.data(), (size_t)C * sizeof(ClassPref));
+  if (B.has_pref) {
+    if (atoms) {
+      ClassPrefT<KB_MAX_W>* d = reinterpret_cast<ClassPrefT<KB_MAX_W>*>(imm.host.data() + oi.class_pref);
+      for (uint32_t k = 0; k < C; ++k) pref_copy(d[k], class_pref[k]);
+    } else memcpy(imm.host.data() + oi.class_pref, B.class_pref.data(), (size_t)C * sizeof(ClassPref));
+  }
   if (pa) {
     unsigned char* ib = imm.host.data(); unsigned char* mb = mut.host.data();
     if (pa->n_keysets && N) memcpy(ib + oi.aff_node_domain, pa->node_domain, (size_t)pa->n_keysets * N * 4);

@@ -81,45 +81,61 @@ struct EvalConf {
 // One task equivalence class: every field of a pending task that predicateFn / the prioritizers /
 // AddTask read.  Tasks of a PodGroup are normally one class.
 //
-// RC: resource dimensions the record holds (its class capacity).  A session with R <= KB_NARROW_R uses the narrow record
-// ClassRecT<KB_NARROW_R> — the layout tests/probe mirrors — and the kernels' narrow instances; a session with up to KB_MAX_R
-// dimensions uses ClassRecT<KB_MAX_R> and the wide instances (the kernels take RC as a template parameter and read the class
-// table through class_table<RC>).  Dimensions >= R are 0.
+// RC: resource dimensions the record holds (its class capacity); WC: 64-bit words of each label / taint / port mask it holds (its
+// word capacity).  A session with R <= KB_NARROW_R and W <= KB_NARROW_W uses the narrow record ClassRecT<KB_NARROW_R,
+// KB_NARROW_W> — the layout tests/probe mirrors — and the kernels' narrow instances; a session with up to KB_MAX_R dimensions uses
+// ClassRecT<KB_MAX_R, KB_NARROW_W>, one with up to KB_MAX_W words (and R <= KB_NARROW_R) ClassRecT<KB_NARROW_R, KB_MAX_W>.  The
+// kernels take the record type as a template parameter and read the class table through class_table<CR>.  Dimensions >= R and
+// words >= W are 0.
 constexpr uint32_t KB_NARROW_R = 8;
-template <uint32_t RC>
+constexpr uint32_t KB_NARROW_W = 4;
+template <uint32_t RC, uint32_t WC = KB_NARROW_W>
 struct ClassRecT {
   static constexpr uint32_t CAP = RC;
+  static constexpr uint32_t WCAP = WC;
   double   initreq[RC];
   double   resreq[RC];
   int64_t  nz_cpu, nz_mem;
-  uint64_t sel_req[KB_MAX_W];
-  uint64_t aff[KB_MAX_AFF_TERMS][KB_MAX_W];
-  uint64_t tol[KB_MAX_W];
-  uint64_t port_own[KB_MAX_W];
-  uint64_t port_conflict[KB_MAX_W];
-  uint64_t aff_own[KB_MAX_W];     // bits an ALLOCATE placement (not a Pipeline) adds to the node's port words: host-level inter-pod
+  uint64_t sel_req[WC];
+  uint64_t aff[KB_MAX_AFF_TERMS][WC];
+  uint64_t tol[WC];
+  uint64_t port_own[WC];
+  uint64_t port_conflict[WC];
+  uint64_t aff_own[WC];           // bits an ALLOCATE placement (not a Pipeline) adds to the node's port words: host-level inter-pod
                                   // anti-affinity encoded as atoms (kb_build.h affinity_as_atoms); all zero otherwise
   uint32_t n_aff;
   uint32_t flags;             // KB_TASK_BEST_EFFORT_QOS only
 };
-// KB_CLASS_R: the capacity of `ClassRec`, i.e. of host code that reads DevSession.classes as ClassRec (the session builder, the
-// evict walk's CPU policy, tests/emu).  The library is built with KB_NARROW_R; tests/emu_wide builds the emulation with KB_MAX_R.
+// KB_CLASS_R / KB_CLASS_W: the capacities of `ClassRec`, i.e. of host code that reads DevSession.classes as ClassRec (the evict
+// walk's CPU policy, tests/emu).  The library is built with KB_NARROW_R / KB_NARROW_W; tests/emu_wide builds the emulation with
+// KB_CLASS_R = KB_MAX_R, tests/emu_wide_atoms with KB_CLASS_W = KB_MAX_W.
 #ifndef KB_CLASS_R
 #define KB_CLASS_R 8
 #endif
+#ifndef KB_CLASS_W
+#define KB_CLASS_W 4
+#endif
 static_assert(KB_CLASS_R == KB_NARROW_R || KB_CLASS_R == KB_MAX_R, "KB_CLASS_R is the narrow or the full capacity");
-using ClassRec = ClassRecT<KB_CLASS_R>;
-using ClassRecWide = ClassRecT<KB_MAX_R>;
+static_assert(KB_CLASS_W == KB_NARROW_W || KB_CLASS_W == KB_MAX_W, "KB_CLASS_W is the narrow or the full word capacity");
+static_assert(KB_CLASS_R == KB_NARROW_R || KB_CLASS_W == KB_NARROW_W, "no record holds both more dimensions and more words");
+using ClassRec = ClassRecT<KB_CLASS_R, KB_CLASS_W>;
+using ClassRecNarrow = ClassRecT<KB_NARROW_R, KB_NARROW_W>;
+using ClassRecWide = ClassRecT<KB_MAX_R, KB_NARROW_W>;        // sessions with R = 9..KB_MAX_R
+using ClassRecAtoms = ClassRecT<KB_NARROW_R, KB_MAX_W>;       // sessions with W = 5..KB_MAX_W (R <= KB_NARROW_R)
+// what the session builder identifies classes by: every dimension ClassRec holds and every mask word a session may have
+using ClassRecBuild = ClassRecT<KB_CLASS_R, KB_MAX_W>;
 
-// Copies a class record into a record of another capacity (dimensions the destination holds beyond the source's become 0)
-template <uint32_t A, uint32_t B>
-inline void class_copy(ClassRecT<A>& d, const ClassRecT<B>& s) {
+// Copies a class record into a record of other capacities (dimensions and words the destination holds beyond the source's become
+// 0; the source's beyond the destination's must be 0)
+template <uint32_t A, uint32_t WA, uint32_t B, uint32_t WB>
+inline void class_copy(ClassRecT<A, WA>& d, const ClassRecT<B, WB>& s) {
   for (uint32_t k = 0; k < A; ++k) { d.initreq[k] = k < B ? s.initreq[k] : 0.0; d.resreq[k] = k < B ? s.resreq[k] : 0.0; }
   d.nz_cpu = s.nz_cpu; d.nz_mem = s.nz_mem;
-  for (uint32_t w = 0; w < KB_MAX_W; ++w) {
-    d.sel_req[w] = s.sel_req[w]; d.tol[w] = s.tol[w]; d.port_own[w] = s.port_own[w]; d.port_conflict[w] = s.port_conflict[w];
-    d.aff_own[w] = s.aff_own[w];
-    for (uint32_t t = 0; t < KB_MAX_AFF_TERMS; ++t) d.aff[t][w] = s.aff[t][w];
+  for (uint32_t w = 0; w < WA; ++w) {
+    const bool in = w < WB;
+    d.sel_req[w] = in ? s.sel_req[w] : 0; d.tol[w] = in ? s.tol[w] : 0; d.port_own[w] = in ? s.port_own[w] : 0;
+    d.port_conflict[w] = in ? s.port_conflict[w] : 0; d.aff_own[w] = in ? s.aff_own[w] : 0;
+    for (uint32_t t = 0; t < KB_MAX_AFF_TERMS; ++t) d.aff[t][w] = in ? s.aff[t][w] : 0;
   }
   d.n_aff = s.n_aff; d.flags = s.flags;
 }
@@ -127,12 +143,28 @@ inline void class_copy(ClassRecT<A>& d, const ClassRecT<B>& s) {
 // Preferred node-affinity terms of a class (NodeAffinityPriority, vendor/.../priorities/node_affinity.go:34-77): requirement
 // atoms that must ALL hold on the node + the term's weight.  Evaluated by cycle_kernel (two-pass scan, kb_pipe.cuh), the
 // per-visit kernels (kb_kernels.cuh), preempt's sweep (kb_evict.h) and the emulation.
-struct ClassPref {
-  uint64_t term[KB_MAX_PREF_TERMS][KB_MAX_W];
+// WC: mask words the record holds, as in ClassRecT.
+template <uint32_t WC = KB_NARROW_W>
+struct ClassPrefT {
+  static constexpr uint32_t WCAP = WC;
+  uint64_t term[KB_MAX_PREF_TERMS][WC];
   int32_t  weight[KB_MAX_PREF_TERMS];
   uint32_t n;
   uint32_t pad[3];
 };
+using ClassPref = ClassPrefT<KB_CLASS_W>;
+using ClassPrefBuild = ClassPrefT<KB_MAX_W>;
+// the preferred terms that go with class records of type CR
+template <class CR> using ClassPrefOf = ClassPrefT<CR::WCAP>;
+
+template <uint32_t WA, uint32_t WB>
+inline void pref_copy(ClassPrefT<WA>& d, const ClassPrefT<WB>& s) {
+  for (uint32_t p = 0; p < KB_MAX_PREF_TERMS; ++p) {
+    for (uint32_t w = 0; w < WA; ++w) d.term[p][w] = w < WB ? s.term[p][w] : 0;
+    d.weight[p] = s.weight[p];
+  }
+  d.n = s.n; d.pad[0] = s.pad[0]; d.pad[1] = s.pad[1]; d.pad[2] = s.pad[2];
+}
 
 // api/resource_info.go:268-274: `l < r || math.Abs(l-r) < diff`.  Evaluated as ONE rounded subtraction and ONE compare:
 //   l <  r  ->  l - r < 0 < diff (a difference of distinct doubles never rounds to zero: gradual underflow), true either way;
@@ -212,8 +244,8 @@ KB_HD int64_t balanced_score(int64_t req_cpu, int64_t cap_cpu, int64_t req_mem, 
 
 // NodeAffinityPriority Map (node_affinity.go:34-77): count = sum of the weights of the preferred terms whose requirement
 // atoms ALL hold on the node (weight 0 terms are skipped)
-template <class NodeAcc>
-KB_HD int32_t pref_count(const ClassPref& cp, const NodeAcc& n, uint32_t W) {
+template <class NodeAcc, uint32_t WC>
+KB_HD int32_t pref_count(const ClassPrefT<WC>& cp, const NodeAcc& n, uint32_t W) {
   int32_t count = 0;
   for (uint32_t p = 0; p < cp.n && p < KB_MAX_PREF_TERMS; ++p) {
     if (cp.weight[p] == 0) continue;

@@ -163,9 +163,12 @@ struct DevSession {
   const double* total_hi; // [R - KB_CLASS_R] dims KB_CLASS_R.. of `total` (sessions with more dims than ClassRec holds), next to the
                           // wide class table in the immutable slab; read through total_of
 };
-// The class table as records of capacity RC (ClassRecT): RC == KB_CLASS_R for a session with R <= KB_CLASS_R, KB_MAX_R above
-template <uint32_t RC>
-KB_HD const ClassRecT<RC>* class_table(const DevSession& S) { return reinterpret_cast<const ClassRecT<RC>*>(S.classes); }
+// The class table as records of type CR (ClassRecT): ClassRec for a session that fits it, ClassRecWide for R > KB_CLASS_R,
+// ClassRecAtoms for W > KB_CLASS_W; the preferred terms (class_pref) in the same word capacity
+template <class CR>
+KB_HD const CR* class_table(const DevSession& S) { return reinterpret_cast<const CR*>(S.classes); }
+template <class CR>
+KB_HD const ClassPrefOf<CR>* pref_table(const DevSession& S) { return reinterpret_cast<const ClassPrefOf<CR>*>(S.class_pref); }
 // drf's totalResource in dimension k (k < R) of a session whose class capacity is RC
 template <uint32_t RC = KB_CLASS_R>
 KB_HD double total_of(const DevSession& S, const uint32_t k) {
@@ -173,8 +176,8 @@ KB_HD double total_of(const DevSession& S, const uint32_t k) {
   return k < KB_CLASS_R ? S.total[k] : S.total_hi[k - KB_CLASS_R];
 }
 constexpr uint32_t KB_MAX_WORLD = 8;
-constexpr uint32_t P2P_RANK_U64 = (2 + 2 * KB_NARROW_R + 6 + 3 * KB_MAX_W) * 32;      // keys + widest record block + flag row
-                                                                                      // (the sharded path takes R <= KB_NARROW_R only)
+constexpr uint32_t P2P_RANK_U64 = (2 + 2 * KB_NARROW_R + 6 + 3 * KB_NARROW_W) * 32;   // keys + widest record block + flag row (the
+                                                                                      // sharded path takes R <= KB_NARROW_R, W <= KB_NARROW_W only)
 constexpr uint32_t P2P_FLAG_OFF = 2 * KB_MAX_WORLD * P2P_RANK_U64;
 constexpr size_t   P2P_REGION_BYTES = ((size_t)P2P_FLAG_OFF + 2 * KB_MAX_WORLD) * 8;
 

@@ -101,7 +101,8 @@ struct kb_engine {
   uint32_t gang_ready = 0;
   uint32_t scan_grid = 1;
   size_t visit_smem = 0, tile_smem = 0, replay_smem = 0, chain_smem = 0;
-  bool wide = false;                        // R > KB_NARROW_R: the kernels' KB_MAX_R instances (wide class records, up to 82 columns)
+  bool wide = false;                        // R > KB_NARROW_R: the kernels' ClassRecWide instances (wide class records, up to 82 columns)
+  bool atoms = false;                       // W > KB_NARROW_W: the kernels' ClassRecAtoms instances (16-word masks, up to 70 columns)
   float load_ms = 0;
   float last_kernel_ms = 0;
   int sm_count = 132;                       // H100 SXM; replaced by the device's multiProcessorCount
@@ -168,55 +169,59 @@ cudaError_t launch_visit(Kernel k, uint32_t grid, size_t smem, cudaStream_t st, 
   return cudaLaunchKernelEx(&cfg, k, D);
 }
 
-// The per-visit launches of one link of the visit chain (allocate view, or backfill with `backfill`), in the class capacity RC of
-// the session.  `pdl`: launch with programmatic dependent launch (graph capture); `extra` counts the prepass launches.
-template <uint32_t RC>
+// The per-visit launches of one link of the visit chain (allocate view, or backfill with `backfill`), in the class record type CR
+// of the session.  `pdl`: launch with programmatic dependent launch (graph capture); `extra` counts the prepass launches.
+template <class CR>
 cudaError_t launch_visit_link(kb_engine* e, const DevSession& D, const bool backfill, const bool pdl, uint32_t* extra) {
   if (D.aff.on) {
     // inter-pod affinity: the priority's passes over the feasible nodes (they return at once for a class without a weight
     // list), then the visit with predicate step 10 / the score term in its scan.  nodeorder is off in backfill: no passes
-    if (backfill) { visit_kernel<1, 1, RC><<<e->scan_grid, SCAN_THREADS, e->visit_smem, e->stream>>>(D); return cudaGetLastError(); }
+    if (backfill) { visit_kernel<1, 1, CR><<<e->scan_grid, SCAN_THREADS, e->visit_smem, e->stream>>>(D); return cudaGetLastError(); }
     if (D.aff.has_weights || D.aff.has_pref) {
       const uint32_t ag = std::max(1u, std::min((e->N + AFF_THREADS - 1) / AFF_THREADS, (uint32_t)e->sm_count * 4u));
       const uint32_t ag1 = std::max(1u, std::min((e->N + AFF_THREADS / 32 - 1) / (AFF_THREADS / 32), (uint32_t)e->sm_count * 8u));   // pass 1: a warp per node
-      aff_prepass_kernel<0, RC><<<ag, AFF_THREADS, 0, e->stream>>>(D);
-      aff_prepass_kernel<1, RC><<<ag1, AFF_THREADS, 0, e->stream>>>(D);
-      aff_prepass_kernel<2, RC><<<ag, AFF_THREADS, 0, e->stream>>>(D);
+      aff_prepass_kernel<0, CR><<<ag, AFF_THREADS, 0, e->stream>>>(D);
+      aff_prepass_kernel<1, CR><<<ag1, AFF_THREADS, 0, e->stream>>>(D);
+      aff_prepass_kernel<2, CR><<<ag, AFF_THREADS, 0, e->stream>>>(D);
       if (extra) *extra += 3;
     }
-    return launch_visit(visit_kernel<0, 1, RC>, e->scan_grid, e->visit_smem, e->stream, D, pdl);
+    return launch_visit(visit_kernel<0, 1, CR>, e->scan_grid, e->visit_smem, e->stream, D, pdl);
   }
-  if (backfill) { visit_kernel<1, 0, RC><<<e->scan_grid, SCAN_THREADS, e->visit_smem, e->stream>>>(D); return cudaGetLastError(); }
-  if (D.overlap) { visit_overlap_kernel<RC><<<e->scan_grid + 1, SCAN_THREADS, e->visit_smem, e->stream>>>(D); return cudaGetLastError(); }
-  if (D.kchain == 2) return launch_visit(visit_chain_kernel<2, RC>, e->scan_grid, e->chain_smem, e->stream, D, pdl);
-  if (D.kchain == 4) return launch_visit(visit_chain_kernel<4, RC>, e->scan_grid, e->chain_smem, e->stream, D, pdl);
-  return launch_visit(visit_kernel<0, 0, RC>, e->scan_grid, e->visit_smem, e->stream, D, pdl);
+  if (backfill) { visit_kernel<1, 0, CR><<<e->scan_grid, SCAN_THREADS, e->visit_smem, e->stream>>>(D); return cudaGetLastError(); }
+  if (D.overlap) { visit_overlap_kernel<CR><<<e->scan_grid + 1, SCAN_THREADS, e->visit_smem, e->stream>>>(D); return cudaGetLastError(); }
+  if (D.kchain == 2) return launch_visit(visit_chain_kernel<2, CR>, e->scan_grid, e->chain_smem, e->stream, D, pdl);
+  if (D.kchain == 4) return launch_visit(visit_chain_kernel<4, CR>, e->scan_grid, e->chain_smem, e->stream, D, pdl);
+  return launch_visit(visit_kernel<0, 0, CR>, e->scan_grid, e->visit_smem, e->stream, D, pdl);
 }
 
-// the wide instances' staging buffers (scan_tpi) fit next to their VisitSmem, down to the widest record at one tile per iteration
-static_assert(((sizeof(VisitSmem<KB_MAX_R>) + 127) / 128) * 128 + 160 * 1024 <= 227 * 1024, "wide VisitSmem + scan_tpi budget");
-static_assert(((sizeof(VisitSmem<KB_MAX_R>) + 127) / 128) * 128 + 2 * (size_t)max_cols<KB_MAX_R>() * TILE_NODES * 8 <= 227 * 1024,
+// the wide and wide-atom instances' staging buffers (scan_tpi) fit next to their VisitSmem, down to the widest record at one tile
+// per iteration
+static_assert(((sizeof(VisitSmem<ClassRecWide>) + 127) / 128) * 128 + 160 * 1024 <= 227 * 1024, "wide VisitSmem + scan_tpi budget");
+static_assert(((sizeof(VisitSmem<ClassRecWide>) + 127) / 128) * 128 + 2 * (size_t)max_cols<ClassRecWide>() * TILE_NODES * 8 <= 227 * 1024,
               "wide VisitSmem + two tiles of the widest record");
+static_assert(((sizeof(VisitSmem<ClassRecAtoms>) + 127) / 128) * 128 + 160 * 1024 <= 227 * 1024, "wide-atom VisitSmem + scan_tpi budget");
+static_assert(((sizeof(VisitSmem<ClassRecAtoms>) + 127) / 128) * 128 + 2 * (size_t)max_cols<ClassRecAtoms>() * TILE_NODES * 8 <= 227 * 1024,
+              "wide-atom VisitSmem + two tiles of the widest record");
 
-// Shared-memory sizes and limits of the kernels of class capacity RC for a session with B.tpi staged tiles of e->tile_smem bytes
-template <uint32_t RC>
+// Shared-memory sizes and limits of the kernels of class record type CR for a session with B.tpi staged tiles of e->tile_smem bytes
+template <class CR>
 cudaError_t set_kernel_smem(kb_engine* e, const uint32_t tpi, const uint32_t kchain) {
-  e->visit_smem = ((sizeof(VisitSmem<RC>) + 127) / 128) * 128 + 2 * (size_t)tpi * e->tile_smem;
+  e->visit_smem = ((sizeof(VisitSmem<CR>) + 127) / 128) * 128 + 2 * (size_t)tpi * e->tile_smem;
   cudaError_t c = cudaSuccess;
-  for (const void* k : {(const void*)visit_kernel<0, 0, RC>, (const void*)visit_kernel<1, 0, RC>, (const void*)visit_kernel<0, 1, RC>,
-                        (const void*)visit_kernel<1, 1, RC>, (const void*)visit_overlap_kernel<RC>})
+  for (const void* k : {(const void*)visit_kernel<0, 0, CR>, (const void*)visit_kernel<1, 0, CR>, (const void*)visit_kernel<0, 1, CR>,
+                        (const void*)visit_kernel<1, 1, CR>, (const void*)visit_overlap_kernel<CR>})
     if (c == cudaSuccess) c = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)e->visit_smem);
   e->chain_smem = 0;
   if (c == cudaSuccess && kchain == 2) {
-    e->chain_smem = chain_smem_header<2, RC>() + 2 * (size_t)tpi * e->tile_smem;
-    c = cudaFuncSetAttribute(visit_chain_kernel<2, RC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)e->chain_smem);
+    e->chain_smem = chain_smem_header<2, CR>() + 2 * (size_t)tpi * e->tile_smem;
+    c = cudaFuncSetAttribute(visit_chain_kernel<2, CR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)e->chain_smem);
   }
   if (c == cudaSuccess && kchain == 4) {
-    e->chain_smem = chain_smem_header<4, RC>() + 2 * (size_t)tpi * e->tile_smem;
-    c = cudaFuncSetAttribute(visit_chain_kernel<4, RC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)e->chain_smem);
+    e->chain_smem = chain_smem_header<4, CR>() + 2 * (size_t)tpi * e->tile_smem;
+    c = cudaFuncSetAttribute(visit_chain_kernel<4, CR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)e->chain_smem);
   }
-  if (c == cudaSuccess) c = cudaFuncSetAttribute(matrix_kernel<RC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)e->tile_smem);
-  if (c == cudaSuccess) c = cudaFuncSetAttribute(best_nodes_kernel<RC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)e->tile_smem);
+  if (c == cudaSuccess) c = cudaFuncSetAttribute(matrix_kernel<CR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)e->tile_smem);
+  if (c == cudaSuccess) c = cudaFuncSetAttribute(best_nodes_kernel<CR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)e->tile_smem);
   return c;
 }
 
@@ -400,9 +405,9 @@ int kb_session_load(kb_engine* e, const kb_snapshot* s, const kb_plugin_conf* co
     const size_t tile_b = (size_t)tile_ncols(s ? s->R : 2, s ? s->W : 1) * TILE_NODES * 8;
     const uint32_t tpi = scan_tpi(s ? s->R : 2, s ? s->W : 1);
     const size_t lim = 227 * 1024;
-    const bool wide = s && s->R > KB_NARROW_R;
-    const size_t h4 = wide ? chain_smem_header<4, KB_MAX_R>() : chain_smem_header<4>();
-    const size_t h2 = wide ? chain_smem_header<2, KB_MAX_R>() : chain_smem_header<2>();
+    const bool wide = s && s->R > KB_NARROW_R, atoms = s && s->W > KB_NARROW_W;
+    const size_t h4 = wide ? chain_smem_header<4, ClassRecWide>() : atoms ? chain_smem_header<4, ClassRecAtoms>() : chain_smem_header<4>();
+    const size_t h2 = wide ? chain_smem_header<2, ClassRecWide>() : atoms ? chain_smem_header<2, ClassRecAtoms>() : chain_smem_header<2>();
     if (kchain == 4 && h4 + 2 * tpi * tile_b > lim) kchain = 2;
     if (kchain == 2 && h2 + 2 * tpi * tile_b > lim) kchain = 1;
   }
@@ -412,9 +417,9 @@ int kb_session_load(kb_engine* e, const kb_snapshot* s, const kb_plugin_conf* co
   // inter-pod affinity (kb_pod_affinity): per-visit kernels on the full table; with world > 1 every rank runs the whole cycle
   // (replicated) unless KB_ENGINE_SHARD asks for the sharded path, which such sessions refuse
   const bool aff_session = s && s->pod_affinity != nullptr;
-  // more resource dimensions than the sharded exchange's records carry (P2P_RANK_U64): replicated unless KB_ENGINE_SHARD asks for
-  // the sharded path, which such sessions refuse (kb_build.h)
-  const bool wide_session = s && s->R > KB_NARROW_R;
+  // more resource dimensions or mask words than the sharded exchange's records carry (P2P_RANK_U64): replicated unless
+  // KB_ENGINE_SHARD asks for the sharded path, which such sessions refuse (kb_build.h)
+  const bool wide_session = s && (s->R > KB_NARROW_R || s->W > KB_NARROW_W);
   const bool pipe_ok = e->pipe_req && e->coop_ok;
   const bool pipe_try = (pipe_ok && (e->world == 1 || !e->shard_req)) || ((aff_session || wide_session) && !e->shard_req);      // = the full table on this rank
   int rc_build = build_session(s, conf, (uint32_t)std::max(1, e->sm_count), B, &be, pipe_try ? 0u : (uint32_t)e->rank,
@@ -478,7 +483,9 @@ int kb_session_load(kb_engine* e, const kb_snapshot* s, const kb_plugin_conf* co
   e->scan_grid = grid;
   e->tile_smem = tile_u64 * 8;
   e->wide = R > KB_NARROW_R;
-  CUDA_TRY(e, e->wide ? set_kernel_smem<KB_MAX_R>(e, B.tpi, B.kchain) : set_kernel_smem<KB_NARROW_R>(e, B.tpi, B.kchain));
+  e->atoms = W > KB_NARROW_W;
+  CUDA_TRY(e, e->wide ? set_kernel_smem<ClassRecWide>(e, B.tpi, B.kchain)
+              : e->atoms ? set_kernel_smem<ClassRecAtoms>(e, B.tpi, B.kchain) : set_kernel_smem<ClassRecNarrow>(e, B.tpi, B.kchain));
   // the cycle is a chain of identical launches: capture BATCH of them into one graph (one host call per batch)
   e->replay_smem = ((sizeof(VisitSmem<>) + 127) / 128) * 128;
   CUDA_TRY(e, cudaFuncSetAttribute(replay_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)e->replay_smem));
@@ -503,8 +510,9 @@ int kb_session_load(kb_engine* e, const kb_snapshot* s, const kb_plugin_conf* co
     bool ok = ce == cudaSuccess;
     for (uint32_t i = 0; ok && i < BATCH; ++i) {
       const bool pdl = e->pdl && (e->world == 1 || e->replicated);
-      if (e->wide) ok = launch_visit_link<KB_MAX_R>(e, e->dev, false, pdl, nullptr) == cudaSuccess;
-      else ok = launch_visit_link<KB_NARROW_R>(e, e->dev, false, pdl, nullptr) == cudaSuccess;
+      if (e->wide) ok = launch_visit_link<ClassRecWide>(e, e->dev, false, pdl, nullptr) == cudaSuccess;
+      else if (e->atoms) ok = launch_visit_link<ClassRecAtoms>(e, e->dev, false, pdl, nullptr) == cudaSuccess;
+      else ok = launch_visit_link<ClassRecNarrow>(e, e->dev, false, pdl, nullptr) == cudaSuccess;
       if (e->world > 1 && !e->dev.p2p && !e->replicated) {      // a replicated rank replays in visit_kernel itself (DevSession.world == 1)
         ok = g_nccl.AllGather(e->dev.sendbuf, e->dev.recvbuf, cnt, kNcclUint64, e->comm, e->stream) == 0;
         replay_kernel<0><<<1, 64, e->replay_smem, e->stream>>>(e->dev);
@@ -590,8 +598,9 @@ int run_action(kb_engine* e, const bool backfill, kb_decision* out, kb_stats* st
       // sharded node axis without peer memory: scan shard -> all-gather (top-32 keys + node records per rank) -> identical replay
       const size_t cnt = (size_t)xchg_u64(e->ncols);
       for (uint32_t i = 0; i < batch; ++i) {
-        if (e->wide) CUDA_TRY(e, launch_visit_link<KB_MAX_R>(e, D, backfill, false, &launches));
-        else CUDA_TRY(e, launch_visit_link<KB_NARROW_R>(e, D, backfill, false, &launches));
+        if (e->wide) CUDA_TRY(e, launch_visit_link<ClassRecWide>(e, D, backfill, false, &launches));
+        else if (e->atoms) CUDA_TRY(e, launch_visit_link<ClassRecAtoms>(e, D, backfill, false, &launches));
+        else CUDA_TRY(e, launch_visit_link<ClassRecNarrow>(e, D, backfill, false, &launches));
         if (e->world > 1 && !D.p2p && !e->replicated) {
           int rc = g_nccl.AllGather(D.sendbuf, D.recvbuf, cnt, kNcclUint64, e->comm, e->stream);
           if (rc != 0) return fail(e, KB_E_NCCL, "ncclAllGather: %s", g_nccl.GetErrorString(rc));
@@ -922,7 +931,8 @@ int kb_predicate_score(kb_engine* e, uint32_t task_lo, uint32_t task_hi, uint8_t
   }
   dim3 grid(e->NT, (task_hi - task_lo + MATRIX_TASKS_PER_CTA - 1) / MATRIX_TASKS_PER_CTA);
   cudaEventRecord(e->ev0, e->stream);
-  if (e->wide) matrix_kernel<KB_MAX_R><<<grid, MATRIX_THREADS, e->tile_smem, e->stream>>>(e->dev, e->d_task_class, task_lo, task_hi, d_fit, d_score);
+  if (e->wide) matrix_kernel<ClassRecWide><<<grid, MATRIX_THREADS, e->tile_smem, e->stream>>>(e->dev, e->d_task_class, task_lo, task_hi, d_fit, d_score);
+  else if (e->atoms) matrix_kernel<ClassRecAtoms><<<grid, MATRIX_THREADS, e->tile_smem, e->stream>>>(e->dev, e->d_task_class, task_lo, task_hi, d_fit, d_score);
   else matrix_kernel<<<grid, MATRIX_THREADS, e->tile_smem, e->stream>>>(e->dev, e->d_task_class, task_lo, task_hi, d_fit, d_score);
   cudaEventRecord(e->ev1, e->stream);
   cudaError_t c = cudaGetLastError();
@@ -952,7 +962,8 @@ int kb_best_nodes(kb_engine* e, uint32_t task_lo, uint32_t task_hi, uint64_t* be
     uint32_t chunks = std::max(1u, std::min(n, (uint32_t)(8 * e->sm_count + e->NT - 1) / std::max(1u, e->NT)));
     dim3 grid(e->NT, chunks);
     cudaEventRecord(e->ev0, e->stream);
-    if (e->wide) best_nodes_kernel<KB_MAX_R><<<grid, MATRIX_THREADS, e->tile_smem, e->stream>>>(e->dev, e->d_task_class, task_lo, task_hi, d_best);
+    if (e->wide) best_nodes_kernel<ClassRecWide><<<grid, MATRIX_THREADS, e->tile_smem, e->stream>>>(e->dev, e->d_task_class, task_lo, task_hi, d_best);
+    else if (e->atoms) best_nodes_kernel<ClassRecAtoms><<<grid, MATRIX_THREADS, e->tile_smem, e->stream>>>(e->dev, e->d_task_class, task_lo, task_hi, d_best);
     else best_nodes_kernel<<<grid, MATRIX_THREADS, e->tile_smem, e->stream>>>(e->dev, e->d_task_class, task_lo, task_hi, d_best);
     cudaEventRecord(e->ev1, e->stream);
     c = cudaGetLastError();

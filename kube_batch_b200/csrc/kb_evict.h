@@ -68,6 +68,7 @@ struct EvictCtl {
   union {                          // master -> workers: the preemptor's class record, in the capacity of the kernel instance
     ClassRec cls;
     ClassRecWide cls_wide;
+    ClassRecAtoms cls_atoms;
   };
 };
 
@@ -97,7 +98,7 @@ struct EvictDev {
   const uint32_t* r_atom_off;    // [n+1] slot -> its entries in r_atom
   const uint32_t* r_atom;        // local atom indices
   const uint32_t* atom_bit;      // [n_atoms] port-word bit of the atom
-  const int32_t*  atom_local;    // [64 * KB_MAX_W] port-word bit -> local atom index, -1 = not counted
+  const int32_t*  atom_local;    // [64 * W] port-word bit -> local atom index, -1 = not counted
   // mutable
   uint8_t*  r_state;             // [n] 0 Running, 1 Releasing (evicted)
   uint32_t* pt_pos;              // [J] tasks popped from preemptorTasks[job]
@@ -206,8 +207,10 @@ KB_HD bool evict_is_victim(const DevSession& S, const EvictDev& E, const Preempt
 // The preferred node-affinity terms preempt's node order reads for this preemptor (util.PrioritizeNodes with NodeAffinityPriority,
 // registered by nodeorder; the condition visit_kernel uses), nullptr when the score has no such term.  reclaim walks ssn.Nodes in
 // order and never scores (reclaim.go:113-115).
-KB_HD const ClassPref* evict_pref(const DevSession& S, const Preemptor& P) {
-  return (P.mode != 0 && S.class_pref != nullptr && S.cf.nodeorder && S.class_pref[P.cls].n != 0) ? &S.class_pref[P.cls] : nullptr;
+// CR: the session's class record type, whose word capacity the preferred terms share (pref_table).
+template <class CR = ClassRec>
+KB_HD const ClassPrefOf<CR>* evict_pref(const DevSession& S, const Preemptor& P) {
+  return (P.mode != 0 && S.class_pref != nullptr && S.cf.nodeorder && pref_table<CR>(S)[P.cls].n != 0) ? &pref_table<CR>(S)[P.cls] : nullptr;
 }
 
 // The weight list InterPodAffinityPriority reads for this preemptor (registered by nodeorder with podaffinity.weight != 0: the
@@ -232,7 +235,7 @@ KB_HD bool evict_pred_ok(const DevSession& S, const CR& c, const uint32_t node) 
 // that passes the predicates — also nodes without Running tasks or eligible victims, and full nodes (preempt never checks Idle) —
 // so this runs on all nodes, not only on those evict_node_key gives a key.  The max starts at 0, so 0 stands for "not counted".
 template <class CR>
-KB_HD uint32_t evict_pref_count(const DevSession& S, const CR& c, const ClassPref& cp, const uint32_t node) {
+KB_HD uint32_t evict_pref_count(const DevSession& S, const CR& c, const ClassPrefOf<CR>& cp, const uint32_t node) {
   if (!evict_pred_ok(S, c, node)) return 0;
   const size_t tile_u64 = (size_t)S.ncols * TILE_NODES;
   TileAcc acc{S.tiles + (size_t)(node / TILE_NODES) * tile_u64, node % TILE_NODES, S.cf.R, S.cf.W};
@@ -246,18 +249,20 @@ KB_HD uint32_t evict_pref_count(const DevSession& S, const CR& c, const ClassPre
 //                 domain of the pods on every node that passes ssn.PredicateFn (aff_pass1_node), amin / amax the min / max of
 //                 aff_count_node over the same nodes (both start at 0).  The pods are NodeInfo.Tasks: an evicted pod stays there
 //                 as Releasing (no count changes), a Pipelined one is added (pipeline_apply).
-struct EvictPrio {
-  const ClassPref* cp;
+template <class CR>
+struct EvictPrioT {
+  const ClassPrefOf<CR>* cp;
   uint32_t pmax;
   const ClassAff* ca;
   long long amin, amax;
 };
+using EvictPrio = EvictPrioT<ClassRec>;
 
 // K1 (+K2 for preempt) + the victim walk of one node: packed key (score, node) if the node's victims cover InitResreq, else 0.
 // The score gains nodeaffinity.weight * (10 * count / pmax) and podaffinity.weight * aff_score (negative weights are already
 // folded into cf.score_bias).
 template <class CR>
-KB_HD uint64_t evict_node_key(const DevSession& S, const EvictDev& E, const Preemptor& P, const CR& c, const EvictPrio& pr,
+KB_HD uint64_t evict_node_key(const DevSession& S, const EvictDev& E, const Preemptor& P, const CR& c, const EvictPrioT<CR>& pr,
                               const uint32_t node, uint32_t* err) {
   const uint32_t R = S.cf.R, W = S.cf.W, n = E.n_run;
   const uint32_t lo = E.node_off[node], hi = E.node_off[node + 1];
@@ -528,11 +533,11 @@ struct CpuExec {
 // A task an earlier allocate / backfill of this cycle Allocated on a node is a member of the groups its class joins (the
 // ClassRec.aff_own bits those placements OR into the record): its atoms' counts on that node go up by one before any eviction
 // reads them.  Only decisions from ctl.fold_step on count: an earlier evicting action of the cycle folded the ones before.
-template <uint32_t RC>
+template <class CR>
 KB_HD void evict_fold_task(const DevSession& S, const EvictDev& E, const uint32_t t) {
   const kb_decision d = S.dec[t];
   if (d.kind != KB_KIND_ALLOCATED || d.node < 0 || d.step < E.ctl->fold_step) return;     // phantom backfill tasks: no node
-  const ClassRecT<RC>& c = class_table<RC>(S)[E.task_class[t]];
+  const CR& c = class_table<CR>(S)[E.task_class[t]];
   for (uint32_t w = 0; w < S.cf.W; ++w)
     for (uint64_t m = c.aff_own[w]; m; m &= m - 1) {
 #if defined(__CUDA_ARCH__)
@@ -545,13 +550,13 @@ KB_HD void evict_fold_task(const DevSession& S, const EvictDev& E, const uint32_
     }
 }
 
-template <uint32_t RC>
+template <class CR>
 KB_HD void evict_scan_job(const DevSession& S, const EvictDev& E, const uint32_t j) {
   int32_t w = E.job_waiting0[j];
   uint32_t first = 0xFFFFFFFFu;
   for (uint32_t i = E.pt_off[j]; i < E.pt_off[j + 1]; ++i) {
     const uint32_t t = E.pt_task[i];
-    if (E.n_atoms) evict_fold_task<RC>(S, E, t);
+    if (E.n_atoms) evict_fold_task<CR>(S, E, t);
     if (S.dec[t].kind == KB_KIND_PIPELINED) w += 1;                  // WaitingTaskNum (job_info.go:396-405)
     if (first == 0xFFFFFFFFu && task_pending(S, t)) first = i - E.pt_off[j];
   }
@@ -564,7 +569,7 @@ KB_HD void evict_init(X& x, const DevSession& S, const EvictDev& E) {
   EvictCtl& ctl = *E.ctl;
   x.sync();
   for (uint32_t j = (uint32_t)x.tid(); j < S.J && !x.jobs_scanned(); j += (uint32_t)x.nthreads()) {
-    evict_scan_job<exec_class_t<X>::CAP>(S, E, j);
+    evict_scan_job<exec_class_t<X>>(S, E, j);
   }
   x.sync();
   if (x.tid() == 0) {
@@ -607,7 +612,7 @@ KB_HD bool try_preemptor(X& x, const DevSession& S, const EvictDev& E, const uin
   if (x.tid() == 0) {
     Preemptor& P = x.pre();
     P.task = task; P.job = job; P.queue = S.job_queue[job]; P.cls = E.task_class[task]; P.mode = mode;
-    if (!ctl.cls_valid || ctl.cls_id != P.cls) { x.cls() = class_table<RC>(S)[P.cls]; ctl.cls_id = P.cls; ctl.cls_valid = 1; }      // 408 B: only when it changes
+    if (!ctl.cls_valid || ctl.cls_id != P.cls) { x.cls() = class_table<exec_class_t<X>>(S)[P.cls]; ctl.cls_id = P.cls; ctl.cls_valid = 1; }      // 408 B: only when it changes
     P.ls = 0.0;
     if (mode != 0 && (E.ec.preempt_fns & EVF_DRF)) {
       double la[RC];
@@ -710,7 +715,7 @@ KB_HD void run_preempt(X& x, const DevSession& S, const EvictDev& E) {
             if (op & 0x80000000u) {
               const uint32_t t = op & 0x7FFFFFFFu;
               Preemptor P; P.task = t; P.job = pj; P.queue = S.job_queue[pj]; P.cls = E.task_class[t]; P.mode = 1; P.ls = 0;
-              pipeline_apply(S, E, P, class_table<exec_class_t<X>::CAP>(S)[P.cls], (uint32_t)S.dec[t].node, true);
+              pipeline_apply(S, E, P, class_table<exec_class_t<X>>(S)[P.cls], (uint32_t)S.dec[t].node, true);
             } else {
               // the slot's node: binary search in node_off
               uint32_t lo = 0, hi = S.N;

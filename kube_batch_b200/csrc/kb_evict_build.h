@@ -107,7 +107,7 @@ inline int build_evict(const kb_snapshot* s, const kb_running* run, const BuiltS
 
   // local atom index of each port-word bit some member's group became (kb_build.h); groups that are no atom are dropped: nobody
   // reads or joins them, so their members' evictions change nothing observable
-  std::vector<int32_t> atom_local(64 * KB_MAX_W, -1);
+  std::vector<int32_t> atom_local((size_t)64 * B.W, -1);          // one entry per port-word bit of the session
   std::vector<uint32_t> atom_bit, r_atom_off(1, 0), r_atom;
   if (lists) {
     std::vector<uint32_t> mine;
@@ -139,7 +139,7 @@ inline int build_evict(const kb_snapshot* s, const kb_running* run, const BuiltS
   EB.oi.pt_task = imm.alloc(T1 * 4); EB.oi.pt_off = imm.alloc(((size_t)J + 1) * 4);
   EB.oi.task_class = imm.alloc(T1 * 4); EB.oi.task_present = imm.alloc(T1 * 4); EB.oi.job_waiting0 = imm.alloc(J1 * 4);
   EB.oi.r_atom_off = imm.alloc(((size_t)n + 1) * 4); EB.oi.r_atom = imm.alloc(std::max<size_t>(1, r_atom.size()) * 4);
-  EB.oi.atom_bit = imm.alloc(std::max(1u, NA) * 4); EB.oi.atom_local = imm.alloc((size_t)64 * KB_MAX_W * 4);
+  EB.oi.atom_bit = imm.alloc(std::max(1u, NA) * 4); EB.oi.atom_local = imm.alloc(atom_local.size() * 4);
   EB.om.r_state = mut.alloc(n1); EB.om.pt_pos = mut.alloc(J1 * 4); EB.om.job_waiting = mut.alloc(J1 * 4);
   EB.om.jheap = mut.alloc(J1 * 4); EB.om.jheap_len = mut.alloc(Q1 * 4); EB.om.qheap = mut.alloc(Q1 * 4); EB.om.queue_map = mut.alloc(Q1 * 4);
   EB.om.q_alloc_present = mut.alloc(Q1 * 4); EB.om.evict_order = mut.alloc(n1 * 4);
@@ -174,7 +174,7 @@ inline int build_evict(const kb_snapshot* s, const kb_running* run, const BuiltS
   if (NA) {
     std::vector<uint32_t> gbase(NG + 1, 0);
     for (uint32_t g = 0; g < NG; ++g) gbase[g + 1] = gbase[g] + pa->keyset_domains[pa->group_keyset[g]];
-    std::vector<int32_t> group_of_atom(64 * KB_MAX_W, -1);
+    std::vector<int32_t> group_of_atom((size_t)64 * B.W, -1);
     for (uint32_t g = 0; g < NG; ++g) if (B.aff_atom_of_group[g] >= 0) group_of_atom[B.aff_atom_of_group[g]] = (int32_t)g;
     int32_t* cnt = (int32_t*)(mb + EB.om.atom_cnt);
     for (uint32_t l = 0; l < NA; ++l) {

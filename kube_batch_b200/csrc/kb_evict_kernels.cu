@@ -58,9 +58,9 @@ __device__ __forceinline__ long long ev_warp_min(const long long v) {
   return (long long)(((unsigned long long)(unsigned)mhi << 32) | mlo);
 }
 
-// the master thread's Exec: single-threaded control, the sweep is farmed out.  RC: class capacity of the session (ClassRecT), the
-// capacity of the mailbox record (EvictCtl.cls / cls_wide) and of the workers' copy
-template <uint32_t RC>
+// the master thread's Exec: single-threaded control, the sweep is farmed out.  CR: class record type of the session (ClassRecT),
+// the type of the mailbox record (EvictCtl.cls / cls_wide / cls_atoms) and of the workers' copy
+template <class CR>
 struct MasterExec {
   EvictCtl* g;
   uint32_t seq;
@@ -70,9 +70,10 @@ struct MasterExec {
   __device__ __forceinline__ uint32_t bcast(uint32_t v) { return v; }
   __device__ __forceinline__ bool jobs_scanned() const { return true; }      // evict_scan_kernel ran before this kernel
   __device__ __forceinline__ void clear_max() {}
-  __device__ __forceinline__ ClassRecT<RC>& cls() {
-    if constexpr (RC == KB_CLASS_R) return g->cls;
-    else return g->cls_wide;
+  __device__ __forceinline__ CR& cls() {
+    if constexpr (std::is_same<CR, ClassRec>::value) return g->cls;
+    else if constexpr (std::is_same<CR, ClassRecWide>::value) return g->cls_wide;
+    else return g->cls_atoms;
   }
   __device__ __forceinline__ Preemptor& pre() { return g->pre; }
   __device__ __forceinline__ void post(const uint32_t pass) {     // one command to every worker CTA, back when all have arrived
@@ -84,26 +85,26 @@ struct MasterExec {
     const uint32_t nw = g->n_workers;
     while (ev_ld_acquire(&g->arrived) < nw) __nanosleep(40);
   }
-  __device__ __forceinline__ uint64_t sweep(const DevSession& S, const EvictDev&, const Preemptor& P, const ClassRecT<RC>&) {
+  __device__ __forceinline__ uint64_t sweep(const DevSession& S, const EvictDev&, const Preemptor& P, const CR&) {
     // preferred node-affinity terms: pass 1 leaves the max count in g->pmax, which is then the sweep's normalisation.  It is
     // taken afresh for every sweep: a Pipeline raises a node's pod count, and max_pods can drop that node together with its count.
     // inter-pod weight list: clear dom_sum, fill it, reduce min / max (and pmax in the same pass) — three commands.
     if (evict_aff(S, P)) { post(2u); post(3u); g->amin = 0ll; g->amax = 0ll; g->pmax = 0u; post(4u); }
-    else if (evict_pref(S, P)) { g->pmax = 0u; post(1u); }
+    else if (evict_pref<CR>(S, P)) { g->pmax = 0u; post(1u); }
     g->red = 0ull;
     post(0u);
     return *((volatile unsigned long long*)&g->red);
   }
 };
 
-template <int PREEMPT, uint32_t RC = KB_NARROW_R>
+template <int PREEMPT, class CR = ClassRecNarrow>
 __global__ void __launch_bounds__(EVICT_THREADS, 1)
 evict_kernel(const __grid_constant__ DevSession S, const __grid_constant__ EvictDev E) {
   EvictCtl* g = E.ctl;
   if (blockIdx.x == gridDim.x - 1) {
     // ---------------- master ----------------
     if (threadIdx.x != 0) return;
-    MasterExec<RC> x{g, 0u};
+    MasterExec<CR> x{g, 0u};
     if (PREEMPT) run_preempt(x, S, E);
     else run_reclaim(x, S, E);
     __threadfence();
@@ -111,9 +112,9 @@ evict_kernel(const __grid_constant__ DevSession S, const __grid_constant__ Evict
     return;
   }
   // ---------------- workers ----------------
-  __shared__ ClassRecT<RC> s_cls;
+  __shared__ CR s_cls;
   __shared__ Preemptor s_pre;
-  __shared__ ClassPref s_pref;                     // preferred node-affinity terms of class s_pref_cls
+  __shared__ ClassPrefOf<CR> s_pref;                     // preferred node-affinity terms of class s_pref_cls
   __shared__ ClassAff s_aff;                       // inter-pod weight list record of class s_aff_cls
   __shared__ uint64_t s_red[EVICT_THREADS / 32];
   __shared__ long long s_mn[EVICT_THREADS / 32], s_mx[EVICT_THREADS / 32];
@@ -139,17 +140,17 @@ evict_kernel(const __grid_constant__ DevSession S, const __grid_constant__ Evict
     {
       const uint32_t* src = reinterpret_cast<const uint32_t*>(&g->cls);
       uint32_t* dst = reinterpret_cast<uint32_t*>(&s_cls);
-      for (uint32_t i = threadIdx.x; i < sizeof(ClassRecT<RC>) / 4; i += EVICT_THREADS) dst[i] = src[i];
+      for (uint32_t i = threadIdx.x; i < sizeof(CR) / 4; i += EVICT_THREADS) dst[i] = src[i];
       const uint32_t* ps = reinterpret_cast<const uint32_t*>(&g->pre);
       uint32_t* pd = reinterpret_cast<uint32_t*>(&s_pre);
       for (uint32_t i = threadIdx.x; i < sizeof(Preemptor) / 4; i += EVICT_THREADS) pd[i] = ps[i];
     }
     __syncthreads();
-    const ClassPref* cp = evict_pref(S, s_pre);    // uniform across the CTA
-    if (cp && s_pref_cls != s_pre.cls) {           // 160 B, only when the class changes
+    const ClassPrefOf<CR>* cp = evict_pref<CR>(S, s_pre);    // uniform across the CTA
+    if (cp && s_pref_cls != s_pre.cls) {           // 160 B (544 B with 16 words), only when the class changes
       const uint32_t* src = reinterpret_cast<const uint32_t*>(cp);
       uint32_t* dst = reinterpret_cast<uint32_t*>(&s_pref);
-      for (uint32_t i = threadIdx.x; i < sizeof(ClassPref) / 4; i += EVICT_THREADS) dst[i] = src[i];
+      for (uint32_t i = threadIdx.x; i < sizeof(ClassPrefOf<CR>) / 4; i += EVICT_THREADS) dst[i] = src[i];
       __syncthreads();
       if (threadIdx.x == 0) s_pref_cls = s_pre.cls;
     }
@@ -236,7 +237,7 @@ evict_kernel(const __grid_constant__ DevSession S, const __grid_constant__ Evict
     }
     uint64_t best = 0;
     uint32_t err = 0;
-    const EvictPrio pr{cp ? &s_pref : nullptr, s_pmax, ca ? &s_aff : nullptr, s_amin, s_amax};
+    const EvictPrioT<CR> pr{cp ? &s_pref : nullptr, s_pmax, ca ? &s_aff : nullptr, s_amin, s_amax};
     for (uint32_t n = blockIdx.x * EVICT_THREADS + threadIdx.x; n < S.N; n += nw * EVICT_THREADS) {
       const uint64_t k = evict_node_key(S, E, s_pre, s_cls, pr, n, &err);
       best = k > best ? k : best;
@@ -266,10 +267,10 @@ evict_kernel(const __grid_constant__ DevSession S, const __grid_constant__ Evict
 }
 
 // evict_init's per-job scan (WaitingTaskNum, first Pending task, the job's Allocated members into the atom counts), one thread per job
-template <uint32_t RC = KB_NARROW_R>
+template <class CR = ClassRecNarrow>
 __global__ void evict_scan_kernel(const __grid_constant__ DevSession S, const __grid_constant__ EvictDev E) {
   const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
-  if (j < S.J) evict_scan_job<RC>(S, E, j);
+  if (j < S.J) evict_scan_job<CR>(S, E, j);
 }
 
 cudaError_t launch_evict(const bool preempt, const DevSession& S, const EvictDev& E, const int sm_count, cudaStream_t stream) {
@@ -283,16 +284,19 @@ cudaError_t launch_evict(const bool preempt, const DevSession& S, const EvictDev
   if (c != cudaSuccess) return c;
   c = cudaMemsetAsync(reinterpret_cast<char*>(E.ctl) + offsetof(EvictCtl, cls_valid), 0, 4, stream);
   if (c != cudaSuccess) return c;
-  // a session with more resource dimensions than the narrow class record holds runs the wide instances (kb_build.h)
-  const bool wide = S.cf.R > KB_NARROW_R;
+  // a session with more resource dimensions or mask words than the narrow class record holds runs the wide or the wide-atom
+  // instances (kb_build.h)
+  const bool wide = S.cf.R > KB_NARROW_R, atoms = S.cf.W > KB_NARROW_W;
   if (S.J) {
-    if (wide) evict_scan_kernel<KB_MAX_R><<<(S.J + 255) / 256, 256, 0, stream>>>(S, E);
+    if (wide) evict_scan_kernel<ClassRecWide><<<(S.J + 255) / 256, 256, 0, stream>>>(S, E);
+    else if (atoms) evict_scan_kernel<ClassRecAtoms><<<(S.J + 255) / 256, 256, 0, stream>>>(S, E);
     else evict_scan_kernel<><<<(S.J + 255) / 256, 256, 0, stream>>>(S, E);
   }
   DevSession s = S; EvictDev ev = E;
   void* args[] = {(void*)&s, (void*)&ev};
-  const void* fn = wide ? (preempt ? (const void*)evict_kernel<1, KB_MAX_R> : (const void*)evict_kernel<0, KB_MAX_R>)
-                        : (preempt ? (const void*)evict_kernel<1> : (const void*)evict_kernel<0>);
+  const void* fn = wide ? (preempt ? (const void*)evict_kernel<1, ClassRecWide> : (const void*)evict_kernel<0, ClassRecWide>)
+                 : atoms ? (preempt ? (const void*)evict_kernel<1, ClassRecAtoms> : (const void*)evict_kernel<0, ClassRecAtoms>)
+                         : (preempt ? (const void*)evict_kernel<1> : (const void*)evict_kernel<0>);
   return cudaLaunchCooperativeKernel(fn, dim3(workers + 1), dim3(EVICT_THREADS), args, 0, stream);
 }
 

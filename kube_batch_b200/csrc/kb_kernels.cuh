@@ -30,9 +30,10 @@ constexpr int MATRIX_THREADS = TILE_NODES;         // matrix / best_nodes kernel
 constexpr int SCAN_WARPS = 16;                     // visit_kernel: 16 warps = up to 4 node tiles in flight per iteration
 constexpr int SCAN_THREADS = SCAN_WARPS * 32;
 constexpr int MAX_TPI = SCAN_WARPS / 4;            // tiles per iteration (4 warps x 32 lanes cover one 128-node tile)
-// widest node record of a session with class capacity RC (2R + 6 + 3W columns): 34 for the narrow instances, 82 for the wide ones
-template <uint32_t RC>
-__host__ __device__ constexpr int max_cols() { return 2 * (int)RC + 6 + 3 * KB_MAX_W; }
+// widest node record of a session with class records of type CR (2R + 6 + 3W columns): 34 for the narrow instances, 82 for the
+// wide ones, 70 for the wide-atom ones
+template <class CR>
+__host__ __device__ constexpr int max_cols() { return 2 * (int)CR::CAP + 6 + 3 * (int)CR::WCAP; }
 constexpr unsigned FULL = 0xFFFFFFFFu;
 
 // ---------------------------------------------------------------------------------------------
@@ -139,16 +140,16 @@ __device__ __forceinline__ uint64_t cta_fold_lists(uint64_t mine, uint64_t (*wli
 // forbidden counter groups >= 64 (ClassAff.xf_*) a scan CTA stages in shared memory: a class forbidden by more reads the rest from L2
 constexpr uint32_t AFF_XF_SMEM = 128;
 
-template <uint32_t RC = KB_NARROW_R>
+template <class CR = ClassRecNarrow>
 struct VisitSmem {
-  ClassRecT<RC> cls;
+  CR cls;
   ClassAff cls_aff;                          // inter-pod affinity record of the class (AFF instantiations only)
   AffX cls_xf[AFF_XF_SMEM];                  // the first AFF_XF_SMEM entries of its forbidden-group list (AFF instantiations only)
-  ClassPref cls_pref;                        // preferred node-affinity terms of the class (AFF instantiations, AffDev.has_pref)
+  ClassPrefOf<CR> cls_pref;                  // preferred node-affinity terms of the class (AFF instantiations, AffDev.has_pref)
   Ctl ctl;
   uint64_t keys[KTOP];                       // merged candidate list of the scan (K3 result)
   uint64_t wlist[SCAN_WARPS][KTOP];          // per-warp lists exchanged through shared memory
-  uint64_t slot[2][max_cols<RC>()][32];      // candidate l: column c of state s at slot[s][c][l] (tile column scheme)
+  uint64_t slot[2][max_cols<CR>()][32];      // candidate l: column c of state s at slot[s][c][l] (tile column scheme)
   uint64_t mbar[2];
   uint32_t is_last;
   uint32_t n_excl;
@@ -186,8 +187,8 @@ __device__ __forceinline__ void store_ctl(Ctl* g, const Ctl& c, int lane) {
 // evaluates ITS candidate's current state for it and the sorted keys go to c.patch (see Ctl).  The caller stores c.
 // CH = 1 (visit_chain_kernel): the floor comes from sm.chain_floor (a patched list's floor is not its 32nd key), the nodes
 // this replay modified are appended to sm.mod and a rescan stop is reported in sm.last_rescan.
-template <int BF, int CH = 0, int AFF = 0, uint32_t RC>
-__device__ __forceinline__ void replay_epilogue(const DevSession& S, VisitSmem<RC>& sm, const int lane, const uint32_t cls_id,
+template <int BF, int CH = 0, int AFF = 0, class CR>
+__device__ __forceinline__ void replay_epilogue(const DevSession& S, VisitSmem<CR>& sm, const int lane, const uint32_t cls_id,
                                                 const uint64_t* rec_base, const uint32_t rec_stride, const uint32_t patch_class,
                                                 const long long t_start, const long long t_scan) {
   // Lane l OWNS candidate l of the merged list: its node record lives in two shared-memory slots
@@ -379,7 +380,7 @@ __device__ __forceinline__ void replay_epilogue(const DevSession& S, VisitSmem<R
     if (placed) {
       if (S.drf_present) {
         double v = 0.0;
-        if ((uint32_t)lane < R && ((S.total_dims_mask >> lane) & 1u)) v = share_of(jalloc, total_of<RC>(S, lane));
+        if ((uint32_t)lane < R && ((S.total_dims_mask >> lane) & 1u)) v = share_of(jalloc, total_of<CR::CAP>(S, lane));
         const uint64_t m = warp_max_u64(double_as_u64(v));
         if (lane == 0) S.job_share[j] = u64_as_double(m);
       }
@@ -395,7 +396,7 @@ __device__ __forceinline__ void replay_epilogue(const DevSession& S, VisitSmem<R
     const long long t_run1 = clock64();
     if (lane == 0) {
       if (reason == STOP_RESCAN) c.rescans += 1;
-      after_run<BF, RC>(S, c, reason, placed, true);
+      after_run<BF, CR::CAP>(S, c, reason, placed, true);
       const long long t_run2 = clock64();
       c.cyc_steps += (unsigned long long)(t_run1 - t_run0);
       c.cyc_ctl += (unsigned long long)(t_run2 - t_run1);
@@ -432,9 +433,9 @@ __device__ __forceinline__ void replay_epilogue(const DevSession& S, VisitSmem<R
     const bool hit = !c.done && c.cur_class == patch_class;
     if (hit) {
       {
-        const uint32_t* src = reinterpret_cast<const uint32_t*>(&class_table<RC>(S)[patch_class]);
+        const uint32_t* src = reinterpret_cast<const uint32_t*>(&class_table<CR>(S)[patch_class]);
         uint32_t* dst = reinterpret_cast<uint32_t*>(&sm.cls);
-        for (uint32_t i = lane; i < sizeof(ClassRecT<RC>) / 4; i += 32) dst[i] = src[i];
+        for (uint32_t i = lane; i < sizeof(CR) / 4; i += 32) dst[i] = src[i];
       }
       __syncwarp();
       uint64_t pk = 0;
@@ -467,8 +468,8 @@ __device__ __forceinline__ void replay_epilogue(const DevSession& S, VisitSmem<R
 // thread 0 of a scanner CTA: start the bulk copies of its first tile group into staging buffer 0 (returns whether the
 // CTA has any group).  The tiles do not depend on the class, so visit_kernel issues this BEFORE it reads the control
 // block; scan_phase is then told that buffer 0 is already in flight.
-template <uint32_t RC>
-__device__ __forceinline__ bool issue_first_group(const DevSession& S, VisitSmem<RC>& sm, uint64_t* tilebuf, const uint32_t scanner_idx) {
+template <class CR>
+__device__ __forceinline__ bool issue_first_group(const DevSession& S, VisitSmem<CR>& sm, uint64_t* tilebuf, const uint32_t scanner_idx) {
   const uint32_t tile_u64 = S.ncols * TILE_NODES;
   const uint32_t tile_bytes = tile_u64 * 8u;
   const uint32_t tpi = S.tpi;
@@ -482,8 +483,8 @@ __device__ __forceinline__ bool issue_first_group(const DevSession& S, VisitSmem
   return true;
 }
 
-template <bool PH = false, int AFF = 0, uint32_t RC>
-__device__ __forceinline__ uint64_t scan_phase(const DevSession& S, VisitSmem<RC>& sm, uint64_t* tilebuf, const uint32_t scanner_idx,
+template <bool PH = false, int AFF = 0, class CR>
+__device__ __forceinline__ uint64_t scan_phase(const DevSession& S, VisitSmem<CR>& sm, uint64_t* tilebuf, const uint32_t scanner_idx,
                                                const uint32_t n_scanners, const uint32_t cls_id, const int tid, const int lane, const int warp,
                                                const bool first_issued = false, const bool pred_dead = false) {
   const uint32_t tile_u64 = S.ncols * TILE_NODES;
@@ -503,9 +504,9 @@ __device__ __forceinline__ uint64_t scan_phase(const DevSession& S, VisitSmem<RC
   if (tid == 0 && n_local > 0 && !first_issued) issue_group(firstg, 0);
   {
     // class record -> shared memory (broadcast reads afterwards) while the first tiles are in flight
-    const uint32_t* src = reinterpret_cast<const uint32_t*>(&class_table<RC>(S)[cls_id]);
+    const uint32_t* src = reinterpret_cast<const uint32_t*>(&class_table<CR>(S)[cls_id]);
     uint32_t* dst = reinterpret_cast<uint32_t*>(&sm.cls);
-    for (uint32_t i = tid; i < sizeof(ClassRecT<RC>) / 4; i += SCAN_THREADS) dst[i] = src[i];
+    for (uint32_t i = tid; i < sizeof(CR) / 4; i += SCAN_THREADS) dst[i] = src[i];
     if (AFF) {
       const uint32_t* as = reinterpret_cast<const uint32_t*>(&S.aff.cls[cls_id]);
       uint32_t* ad = reinterpret_cast<uint32_t*>(&sm.cls_aff);
@@ -516,8 +517,8 @@ __device__ __forceinline__ uint64_t scan_phase(const DevSession& S, VisitSmem<RC
       }
       uint32_t* pd = reinterpret_cast<uint32_t*>(&sm.cls_pref);
       if (S.aff.has_pref) {
-        const uint32_t* ps = reinterpret_cast<const uint32_t*>(&S.class_pref[cls_id]);
-        for (uint32_t i = tid; i < sizeof(ClassPref) / 4; i += SCAN_THREADS) pd[i] = ps[i];
+        const uint32_t* ps = reinterpret_cast<const uint32_t*>(&pref_table<CR>(S)[cls_id]);
+        for (uint32_t i = tid; i < sizeof(ClassPrefOf<CR>) / 4; i += SCAN_THREADS) pd[i] = ps[i];
       } else if (tid == 0) sm.cls_pref.n = 0;
     }
   }
@@ -650,14 +651,15 @@ __device__ __forceinline__ void shadow_prefetch(const DevSession& S, const Ctl& 
 // ---------------------------------------------------------------------------------------------
 // visit_kernel
 // ---------------------------------------------------------------------------------------------
-// RC: class capacity of the session (KB_NARROW_R, or KB_MAX_R for R > KB_NARROW_R): the class record and the candidate slots
-template <int BF, int AFF = 0, uint32_t RC = KB_NARROW_R>
+// CR: class record type of the session (ClassRecNarrow, ClassRecWide for R > KB_NARROW_R, ClassRecAtoms for W > KB_NARROW_W): the
+// class record, its preferred terms and the candidate slots
+template <int BF, int AFF = 0, class CR = ClassRecNarrow>
 __global__ void __launch_bounds__(SCAN_THREADS)
 visit_kernel(const __grid_constant__ DevSession S) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   // layout: [VisitSmem][pad to 128][tile buffer 0][tile buffer 1]
-  VisitSmem<RC>& sm = *reinterpret_cast<VisitSmem<RC>*>(smem_raw);
-  uint64_t* tilebuf = reinterpret_cast<uint64_t*>(smem_raw + ((sizeof(VisitSmem<RC>) + 127) / 128) * 128);
+  VisitSmem<CR>& sm = *reinterpret_cast<VisitSmem<CR>*>(smem_raw);
+  uint64_t* tilebuf = reinterpret_cast<uint64_t*>(smem_raw + ((sizeof(VisitSmem<CR>) + 127) / 128) * 128);
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   Ctl* gctl = S.ctl;
@@ -846,16 +848,16 @@ visit_kernel(const __grid_constant__ DevSession S) {
 // global tiles (L2 resident); feasible = K1 + predicate step 10, exactly the scan's test.
 // ---------------------------------------------------------------------------------------------
 constexpr int AFF_THREADS = 256;
-template <int PHASE, uint32_t RC = KB_NARROW_R>
+template <int PHASE, class CR = ClassRecNarrow>
 __global__ void __launch_bounds__(AFF_THREADS)
 aff_prepass_kernel(const __grid_constant__ DevSession S) {
-  __shared__ ClassRecT<RC> scls;
+  __shared__ CR scls;
   __shared__ ClassAff sca;
   __shared__ AffX sxf[AFF_XF_SMEM];
   if (__ldcg(&S.ctl->done) || !S.cf.nodeorder) return;
   const uint32_t cls_id = __ldcg(&S.ctl->cur_class);
   const bool wts = S.aff.cls[cls_id].w_cnt != 0;
-  const bool prf = S.aff.has_pref && S.class_pref[cls_id].n != 0;        // NodeAffinityPriority: max count over the feasible nodes
+  const bool prf = S.aff.has_pref && pref_table<CR>(S)[cls_id].n != 0;        // NodeAffinityPriority: max count over the feasible nodes
   if (!wts && !prf) return;
   const uint32_t gtid = blockIdx.x * blockDim.x + threadIdx.x, nthr = gridDim.x * blockDim.x;
   if (PHASE == 0) {
@@ -864,16 +866,16 @@ aff_prepass_kernel(const __grid_constant__ DevSession S) {
     return;
   }
   if (PHASE == 1 && !wts) return;
-  __shared__ ClassPref scp;
+  __shared__ ClassPrefOf<CR> scp;
   if (prf) {
-    const uint32_t* ps = reinterpret_cast<const uint32_t*>(&S.class_pref[cls_id]);
+    const uint32_t* ps = reinterpret_cast<const uint32_t*>(&pref_table<CR>(S)[cls_id]);
     uint32_t* pd = reinterpret_cast<uint32_t*>(&scp);
-    for (uint32_t i = threadIdx.x; i < sizeof(ClassPref) / 4; i += blockDim.x) pd[i] = ps[i];
+    for (uint32_t i = threadIdx.x; i < sizeof(ClassPrefOf<CR>) / 4; i += blockDim.x) pd[i] = ps[i];
   }
   {
-    const uint32_t* src = reinterpret_cast<const uint32_t*>(&class_table<RC>(S)[cls_id]);
+    const uint32_t* src = reinterpret_cast<const uint32_t*>(&class_table<CR>(S)[cls_id]);
     uint32_t* dst = reinterpret_cast<uint32_t*>(&scls);
-    for (uint32_t i = threadIdx.x; i < sizeof(ClassRecT<RC>) / 4; i += blockDim.x) dst[i] = src[i];
+    for (uint32_t i = threadIdx.x; i < sizeof(CR) / 4; i += blockDim.x) dst[i] = src[i];
     const uint32_t* as = reinterpret_cast<const uint32_t*>(&S.aff.cls[cls_id]);
     uint32_t* ad = reinterpret_cast<uint32_t*>(&sca);
     for (uint32_t i = threadIdx.x; i < sizeof(ClassAff) / 4; i += blockDim.x) ad[i] = as[i];
@@ -936,21 +938,21 @@ aff_prepass_kernel(const __grid_constant__ DevSession S) {
 // is re-evaluated; keys are unique (node index), so "best >= floor" certifies a pick exactly as in visit_kernel.
 // A wrong prediction only wastes the look-ahead evaluation.  tests/emu mirrors this protocol (emu_launch_chain).
 // ---------------------------------------------------------------------------------------------
-template <int K, uint32_t RC = KB_NARROW_R>
+template <int K, class CR = ClassRecNarrow>
 struct ChainSmem {
-  ClassRecT<RC> cls[K];
+  CR cls[K];
   uint32_t cls_id[K];
   uint64_t keys[K][KTOP];                    // merged list per class (launch-start state)
   uint64_t fold[2][K][SCAN_WARPS][KTOP];     // ping-pong buffers of the fold rounds
 };
-template <int K, uint32_t RC = KB_NARROW_R>
+template <int K, class CR = ClassRecNarrow>
 __host__ __device__ constexpr size_t chain_smem_header() {
-  return ((sizeof(VisitSmem<RC>) + 127) / 128) * 128 + ((sizeof(ChainSmem<K, RC>) + 127) / 128) * 128;
+  return ((sizeof(VisitSmem<CR>) + 127) / 128) * 128 + ((sizeof(ChainSmem<K, CR>) + 127) / 128) * 128;
 }
 
 // one fold round over lists of `nK` classes: n lists per class in buf[cur] -> n/2 in buf[cur^1]; jobs spread over the warps
-template <int K, uint32_t RC>
-__device__ __forceinline__ void chain_fold_round(ChainSmem<K, RC>& cs, const int cur, const int n, const int nK, const int warp, const int lane) {
+template <int K, class CR>
+__device__ __forceinline__ void chain_fold_round(ChainSmem<K, CR>& cs, const int cur, const int n, const int nK, const int warp, const int lane) {
   const int half = n >> 1, jobs = nK * half;
   for (int t = warp; t < jobs; t += SCAN_WARPS) {
     const int k = t / half, i = t - k * half;
@@ -959,13 +961,13 @@ __device__ __forceinline__ void chain_fold_round(ChainSmem<K, RC>& cs, const int
   __syncthreads();
 }
 
-template <int K, uint32_t RC = KB_NARROW_R>
+template <int K, class CR = ClassRecNarrow>
 __global__ void __launch_bounds__(SCAN_THREADS)
 visit_chain_kernel(const __grid_constant__ DevSession S) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
-  VisitSmem<RC>& sm = *reinterpret_cast<VisitSmem<RC>*>(smem_raw);
-  ChainSmem<K, RC>& cs = *reinterpret_cast<ChainSmem<K, RC>*>(smem_raw + ((sizeof(VisitSmem<RC>) + 127) / 128) * 128);
-  uint64_t* tilebuf = reinterpret_cast<uint64_t*>(smem_raw + chain_smem_header<K, RC>());
+  VisitSmem<CR>& sm = *reinterpret_cast<VisitSmem<CR>*>(smem_raw);
+  ChainSmem<K, CR>& cs = *reinterpret_cast<ChainSmem<K, CR>*>(smem_raw + ((sizeof(VisitSmem<CR>) + 127) / 128) * 128);
+  uint64_t* tilebuf = reinterpret_cast<uint64_t*>(smem_raw + chain_smem_header<K, CR>());
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   Ctl* gctl = S.ctl;
@@ -994,9 +996,9 @@ visit_chain_kernel(const __grid_constant__ DevSession S) {
   };
   if (tid == 0 && n_local > 0) issue_group(firstg, 0);
   for (int k = 0; k < nK; ++k) {
-    const uint32_t* src = reinterpret_cast<const uint32_t*>(&class_table<RC>(S)[cs.cls_id[k]]);
+    const uint32_t* src = reinterpret_cast<const uint32_t*>(&class_table<CR>(S)[cs.cls_id[k]]);
     uint32_t* dst = reinterpret_cast<uint32_t*>(&cs.cls[k]);
-    for (uint32_t i = tid; i < sizeof(ClassRecT<RC>) / 4; i += SCAN_THREADS) dst[i] = src[i];
+    for (uint32_t i = tid; i < sizeof(CR) / 4; i += SCAN_THREADS) dst[i] = src[i];
   }
   __syncthreads();
   const uint32_t sub = (uint32_t)warp >> 2, part = (uint32_t)warp & 3u;
@@ -1031,7 +1033,7 @@ visit_chain_kernel(const __grid_constant__ DevSession S) {
   for (int k = 0; k < K; ++k) if (k < nK) cs.fold[0][k][warp][lane] = mylist[k];
   __syncthreads();
   int cur = 0;
-  for (int n = SCAN_WARPS; n > 1; n >>= 1) { chain_fold_round<K, RC>(cs, cur, n, nK, warp, lane); cur ^= 1; }
+  for (int n = SCAN_WARPS; n > 1; n >>= 1) { chain_fold_round<K, CR>(cs, cur, n, nK, warp, lane); cur ^= 1; }
   const uint32_t G = gridDim.x;
   if (warp < nK) {
     const uint64_t v = cs.fold[cur][warp][0][lane];
@@ -1079,14 +1081,14 @@ visit_chain_kernel(const __grid_constant__ DevSession S) {
     }
     __syncthreads();
     cur = 0;
-    for (int n = P; n > 1; n >>= 1) { chain_fold_round<K, RC>(cs, cur, n, nK, warp, lane); cur ^= 1; }
+    for (int n = P; n > 1; n >>= 1) { chain_fold_round<K, CR>(cs, cur, n, nK, warp, lane); cur ^= 1; }
     if (warp < nK) cs.keys[warp][lane] = cs.fold[cur][warp][0][lane];
   }
   if (warp == 0) { __syncwarp(); sm.keys[lane] = cs.keys[0][lane]; if (lane == 0) sm.chain_floor = cs.keys[0][KTOP - 1]; }
   {
     const uint32_t* src = reinterpret_cast<const uint32_t*>(&cs.cls[0]);
     uint32_t* dst = reinterpret_cast<uint32_t*>(&sm.cls);
-    for (uint32_t i = tid; i < sizeof(ClassRecT<RC>) / 4; i += SCAN_THREADS) dst[i] = src[i];
+    for (uint32_t i = tid; i < sizeof(CR) / 4; i += SCAN_THREADS) dst[i] = src[i];
   }
   if (warp == SCAN_WARPS - 1) {
 #pragma unroll
@@ -1204,7 +1206,7 @@ visit_chain_kernel(const __grid_constant__ DevSession S) {
     {
       const uint32_t* src = reinterpret_cast<const uint32_t*>(&cs.cls[nk]);
       uint32_t* dst = reinterpret_cast<uint32_t*>(&sm.cls);
-      for (uint32_t i = lane; i < sizeof(ClassRecT<RC>) / 4; i += 32) dst[i] = src[i];
+      for (uint32_t i = lane; i < sizeof(CR) / 4; i += 32) dst[i] = src[i];
     }
     used |= 1u << nk;
     kcur = nk;
@@ -1230,12 +1232,12 @@ visit_chain_kernel(const __grid_constant__ DevSession S) {
 // patched from the replayer's own up-to-date copy.  A wrong prediction only costs the overlap of one launch.
 // ---------------------------------------------------------------------------------------------
 
-template <uint32_t RC = KB_NARROW_R>
+template <class CR = ClassRecNarrow>
 __global__ void __launch_bounds__(SCAN_THREADS)
 visit_overlap_kernel(const __grid_constant__ DevSession S) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
-  VisitSmem<RC>& sm = *reinterpret_cast<VisitSmem<RC>*>(smem_raw);
-  uint64_t* tilebuf = reinterpret_cast<uint64_t*>(smem_raw + ((sizeof(VisitSmem<RC>) + 127) / 128) * 128);
+  VisitSmem<CR>& sm = *reinterpret_cast<VisitSmem<CR>*>(smem_raw);
+  uint64_t* tilebuf = reinterpret_cast<uint64_t*>(smem_raw + ((sizeof(VisitSmem<CR>) + 127) / 128) * 128);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   Ctl* gctl = S.ctl;
   if (*((volatile uint32_t*)&gctl->done)) return;
@@ -1265,9 +1267,9 @@ visit_overlap_kernel(const __grid_constant__ DevSession S) {
       const uint32_t cls_id = c.list_class;
       const uint32_t patch_class = c.n_excl > 0 ? c.scan_class : 0xFFFFFFFEu;   // 0xFFFFFFFE never matches a class
       {
-        const uint32_t* src = reinterpret_cast<const uint32_t*>(&class_table<RC>(S)[cls_id]);
+        const uint32_t* src = reinterpret_cast<const uint32_t*>(&class_table<CR>(S)[cls_id]);
         uint32_t* dst = reinterpret_cast<uint32_t*>(&sm.cls);
-        for (uint32_t i = lane; i < sizeof(ClassRecT<RC>) / 4; i += 32) dst[i] = src[i];
+        for (uint32_t i = lane; i < sizeof(CR) / 4; i += 32) dst[i] = src[i];
       }
       sm.keys[lane] = c.list[lane];
       __syncwarp();
@@ -1361,7 +1363,7 @@ template <int BF>
 __global__ void __launch_bounds__(64)
 replay_kernel(const __grid_constant__ DevSession S) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
-  VisitSmem<>& sm = *reinterpret_cast<VisitSmem<>*>(smem_raw);      // narrow sessions only: the sharded path takes R <= KB_NARROW_R
+  VisitSmem<>& sm = *reinterpret_cast<VisitSmem<>*>(smem_raw);      // narrow sessions only: the sharded path takes R <= KB_NARROW_R, W <= KB_NARROW_W
   const int lane = threadIdx.x & 31;
   Ctl* gctl = S.ctl;
   if (*((volatile uint32_t*)&gctl->done)) return;
@@ -1493,12 +1495,12 @@ __global__ void seed_backfill_kernel(const Ctl* __restrict__ main_ctl, Ctl* __re
 // ---------------------------------------------------------------------------------------------
 constexpr int MATRIX_TASKS_PER_CTA = 32;
 
-template <uint32_t RC = KB_NARROW_R>
+template <class CR = ClassRecNarrow>
 __global__ void __launch_bounds__(MATRIX_THREADS)
 matrix_kernel(const __grid_constant__ DevSession S, const uint32_t* __restrict__ task_class, uint32_t task_lo, uint32_t task_hi,
               uint8_t* __restrict__ fit, double* __restrict__ score) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
-  __shared__ ClassRecT<RC> cls;
+  __shared__ CR cls;
   __shared__ uint64_t mbar;
   uint64_t* tilebuf = reinterpret_cast<uint64_t*>(smem_raw);
   const int tid = threadIdx.x;
@@ -1517,9 +1519,9 @@ matrix_kernel(const __grid_constant__ DevSession S, const uint32_t* __restrict__
   for (uint32_t t = t0; t < t1; ++t) {
     __syncthreads();
     {
-      const uint32_t* src = reinterpret_cast<const uint32_t*>(&class_table<RC>(S)[task_class[t]]);
+      const uint32_t* src = reinterpret_cast<const uint32_t*>(&class_table<CR>(S)[task_class[t]]);
       uint32_t* dst = reinterpret_cast<uint32_t*>(&cls);
-      for (uint32_t i = tid; i < sizeof(ClassRecT<RC>) / 4; i += MATRIX_THREADS) dst[i] = src[i];
+      for (uint32_t i = tid; i < sizeof(CR) / 4; i += MATRIX_THREADS) dst[i] = src[i];
     }
     __syncthreads();
     if (node < S.N) {
@@ -1535,12 +1537,12 @@ matrix_kernel(const __grid_constant__ DevSession S, const uint32_t* __restrict__
 }
 
 // K1+K2+K3 fused: per-task best packed key over ALL nodes in one launch.
-template <uint32_t RC = KB_NARROW_R>
+template <class CR = ClassRecNarrow>
 __global__ void __launch_bounds__(MATRIX_THREADS)
 best_nodes_kernel(const __grid_constant__ DevSession S, const uint32_t* __restrict__ task_class, uint32_t task_lo, uint32_t task_hi,
                   unsigned long long* __restrict__ best_key) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
-  __shared__ ClassRecT<RC> cls;
+  __shared__ CR cls;
   __shared__ uint64_t mbar;
   uint64_t* tilebuf = reinterpret_cast<uint64_t*>(smem_raw);
   const int tid = threadIdx.x, lane = tid & 31;
@@ -1562,9 +1564,9 @@ best_nodes_kernel(const __grid_constant__ DevSession S, const uint32_t* __restri
     const uint32_t cid = task_class[t];
     if (cid != cur_cls) {            // tasks of a PodGroup share a class: reload only on change (uniform branch)
       __syncthreads();
-      const uint32_t* src = reinterpret_cast<const uint32_t*>(&class_table<RC>(S)[cid]);
+      const uint32_t* src = reinterpret_cast<const uint32_t*>(&class_table<CR>(S)[cid]);
       uint32_t* dst = reinterpret_cast<uint32_t*>(&cls);
-      for (uint32_t i = tid; i < sizeof(ClassRecT<RC>) / 4; i += MATRIX_THREADS) dst[i] = src[i];
+      for (uint32_t i = tid; i < sizeof(CR) / 4; i += MATRIX_THREADS) dst[i] = src[i];
       __syncthreads();
       cur_cls = cid;
     }

@@ -32,6 +32,7 @@
 #include <vector>
 
 #include "../../include/kbgpu.h"
+#include "../csrc/kb_core.h"      // KB_NARROW_R / KB_NARROW_W: the capacities no kernel instance exceeds both of
 
 namespace kb {
 
@@ -669,7 +670,10 @@ inline Flat Flatten(const framework::Session& ssn) {
   for (auto& jk : ssn.Jobs) for (auto& tk : jk.second->Tasks) for (auto& h : tk.second->pod->HostPorts) if (h.Port > 0) portAtoms.emplace(san(h), (uint32_t)portAtoms.size());
   size_t need = std::max({atoms.reqs.size(), taintAtoms.size(), portAtoms.size(), (size_t)1});
   f.W = (uint32_t)((need + 63) / 64);
-  if (f.W > KB_MAX_W) throw Unsupported(std::to_string(need) + " label / taint / port atoms > 64 x KB_MAX_W");
+  if (f.W > KB_MAX_W) throw Unsupported(std::to_string(need) + " label / taint / port atoms > 64 x KB_MAX_W (" + std::to_string(KB_MAX_W) + ")");
+  if (f.R > kb::KB_NARROW_R && f.W > kb::KB_NARROW_W)
+    throw Unsupported(std::to_string(f.R) + " resource dimensions > KB_NARROW_R (" + std::to_string(kb::KB_NARROW_R) + ") with " + std::to_string(need) +
+                      " atoms > 64 x KB_NARROW_W (" + std::to_string(kb::KB_NARROW_W) + ")");
   const uint32_t R = f.R, W = f.W, N = f.N, T = f.T, J = f.J, Q = f.Q;
   auto setbit = [](std::vector<uint64_t>& a, size_t stride, size_t i, uint32_t atom) { a[(atom / 64) * stride + i] |= 1ull << (atom % 64); };
   // nodes
