@@ -228,6 +228,7 @@ struct BuiltSession {
   OffImm oi{};
   HostConf hc;
   uint32_t R = 0, W = 0, N = 0, T = 0, J = 0, Q = 0, C = 0, NT = 0, ncols = 0, To = 0, grid = 1;
+  RecKind rec = RecKind::Own;        // the record type of the class tables and preferred terms: rec_kind(R, W)
   uint32_t total_dims_mask = 3;
   double total[KB_MAX_R] = {0};
   std::vector<int32_t> job_min_avail;
@@ -915,10 +916,9 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
   om.recvbuf = mut.alloc((size_t)std::max(1u, world) * xchg_u64(ncols) * 8);
   om.bf_job_pos = mut.alloc((size_t)std::max(1u, J) * 4);
   om.bf_ctl = mut.alloc(sizeof(Ctl));
-  // the session's record type: ClassRecWide for R > KB_CLASS_R, ClassRecAtoms for W > KB_CLASS_W, else ClassRec
-  const bool atoms = W > KB_CLASS_W;
-  const size_t class_bytes = RH ? sizeof(ClassRecWide) : atoms ? sizeof(ClassRecAtoms) : sizeof(ClassRec);
-  const size_t pref_bytes = atoms ? sizeof(ClassPrefT<KB_MAX_W>) : sizeof(ClassPref);
+  B.rec = rec_kind(R, W);
+  const size_t class_bytes = with_rec(B.rec, [](auto t) { return sizeof(typename decltype(t)::type); });
+  const size_t pref_bytes = with_rec(B.rec, [](auto t) { return sizeof(ClassPrefOf<typename decltype(t)::type>); });
   oi.classes = imm.alloc((size_t)C * class_bytes);
   oi.total_hi = imm.alloc((size_t)std::max(1u, RH) * 8);
   oi.ord_task = imm.alloc((size_t)std::max(1u, To) * 4);
@@ -1009,32 +1009,28 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
 
   // ---------------- immutable job / queue / class tables ----------------
   // the class table in the session's record type; a wide record joins the narrow part with its dims past KB_CLASS_R
-  auto write_as = [&](auto* tab, const bool backfill) {
-    using CR = typename std::remove_pointer<decltype(tab)>::type;
-    for (uint32_t k = 0; k < C; ++k) {
-      CR w;
-      memset(&w, 0, sizeof w);
-      class_copy(w, classes[k]);
-      for (uint32_t r = KB_CLASS_R; r < R && r < CR::CAP; ++r) {
-        w.initreq[r] = class_hi[(size_t)k * 2 * RH + (r - KB_CLASS_R)];
-        w.resreq[r] = class_hi[(size_t)k * 2 * RH + RH + (r - KB_CLASS_R)];
-      }
-      if (backfill) for (uint32_t r = 0; r < CR::CAP; ++r) w.initreq[r] = w.resreq[r];
-      memcpy(&tab[k], &w, sizeof w);
-    }
-  };
   auto write_classes = [&](unsigned char* dst, const bool backfill) {
-    if (RH) write_as(reinterpret_cast<ClassRecWide*>(dst), backfill);
-    else if (atoms) write_as(reinterpret_cast<ClassRecAtoms*>(dst), backfill);
-    else write_as(reinterpret_cast<ClassRec*>(dst), backfill);
+    with_rec(B.rec, [&](auto t) {
+      using CR = typename decltype(t)::type;
+      for (uint32_t k = 0; k < C; ++k) {
+        CR w;
+        memset(&w, 0, sizeof w);
+        class_copy(w, classes[k]);
+        for (uint32_t r = KB_CLASS_R; r < R && r < CR::CAP; ++r) {
+          w.initreq[r] = class_hi[(size_t)k * 2 * RH + (r - KB_CLASS_R)];
+          w.resreq[r] = class_hi[(size_t)k * 2 * RH + RH + (r - KB_CLASS_R)];
+        }
+        if (backfill) for (uint32_t r = 0; r < CR::CAP; ++r) w.initreq[r] = w.resreq[r];
+        memcpy(dst + k * sizeof w, &w, sizeof w);
+      }
+    });
   };
   write_classes(imm.host.data() + oi.classes, false);
-  if (B.has_pref) {
-    if (atoms) {
-      ClassPrefT<KB_MAX_W>* d = reinterpret_cast<ClassPrefT<KB_MAX_W>*>(imm.host.data() + oi.class_pref);
+  if (B.has_pref)
+    with_rec(B.rec, [&](auto t) {
+      auto* d = reinterpret_cast<ClassPrefOf<typename decltype(t)::type>*>(imm.host.data() + oi.class_pref);
       for (uint32_t k = 0; k < C; ++k) pref_copy(d[k], class_pref[k]);
-    } else memcpy(imm.host.data() + oi.class_pref, B.class_pref.data(), (size_t)C * sizeof(ClassPref));
-  }
+    });
   if (pa) {
     unsigned char* ib = imm.host.data(); unsigned char* mb = mut.host.data();
     if (pa->n_keysets && N) memcpy(ib + oi.aff_node_domain, pa->node_domain, (size_t)pa->n_keysets * N * 4);
@@ -1124,8 +1120,7 @@ inline int build_session(const kb_snapshot* s, const kb_plugin_conf* conf, uint3
     for (uint32_t i = 0; i < RH; ++i) reinterpret_cast<double*>(imm.host.data() + oi.total_hi)[i] = B.total[KB_CLASS_R + i];
   for (uint32_t j = 0; j < J; ++j) {
     if (!hc.drf_present) H.job_share[j] = 0.0;
-    else if (RH) update_job_share<KB_MAX_R>(H, j);
-    else update_job_share(H, j);
+    else with_rec(B.rec, [&](auto t) { update_job_share<decltype(t)::type::CAP>(H, j); });
   }
 
   // proportion OnSessionOpen (proportion.go:58-154)

@@ -125,6 +125,22 @@ using ClassRecAtoms = ClassRecT<KB_NARROW_R, KB_MAX_W>;       // sessions with W
 // what the session builder identifies classes by: every dimension ClassRec holds and every mask word a session may have
 using ClassRecBuild = ClassRecT<KB_CLASS_R, KB_MAX_W>;
 
+// The record a session of R dimensions and W words runs, decided here only, so that the class table's writer and the kernels'
+// launch sites cannot disagree: the build's own ClassRec when the session fits it, else the wide or the wide-atom record
+enum class RecKind { Own, Wide, Atoms };
+inline RecKind rec_kind(uint32_t R, uint32_t W) { return R > KB_CLASS_R ? RecKind::Wide : W > KB_CLASS_W ? RecKind::Atoms : RecKind::Own; }
+template <class CR> struct RecTag { using type = CR; };
+// f(RecTag<CR>{}) with the record type CR of `kind`; no default arm, so that -Wswitch flags a kind without one
+template <class F>
+inline auto with_rec(RecKind kind, F&& f) {
+  switch (kind) {
+    case RecKind::Own: return f(RecTag<ClassRec>{});
+    case RecKind::Wide: return f(RecTag<ClassRecWide>{});
+    case RecKind::Atoms: return f(RecTag<ClassRecAtoms>{});
+  }
+  __builtin_unreachable();
+}
+
 // Copies a class record into a record of other capacities (dimensions and words the destination holds beyond the source's become
 // 0; the source's beyond the destination's must be 0)
 template <uint32_t A, uint32_t WA, uint32_t B, uint32_t WB>

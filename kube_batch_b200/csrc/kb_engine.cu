@@ -101,8 +101,6 @@ struct kb_engine {
   uint32_t gang_ready = 0;
   uint32_t scan_grid = 1;
   size_t visit_smem = 0, tile_smem = 0, replay_smem = 0, chain_smem = 0;
-  bool wide = false;                        // R > KB_NARROW_R: the kernels' ClassRecWide instances (wide class records, up to 82 columns)
-  bool atoms = false;                       // W > KB_NARROW_W: the kernels' ClassRecAtoms instances (16-word masks, up to 70 columns)
   float load_ms = 0;
   float last_kernel_ms = 0;
   int sm_count = 132;                       // H100 SXM; replaced by the device's multiProcessorCount
@@ -137,6 +135,7 @@ struct kb_engine {
   double watchdog_s = 30.0;                 // a cycle_kernel that has not finished after this long is reported (with the progress words) and the process aborts: a hung cooperative kernel cannot be cancelled
   cudaGraph_t graph = nullptr;         // BATCH visit_kernel launches, captured once per distinct DevSession
   cudaGraphExec_t graph_exec = nullptr;
+  uint32_t graph_launches = 0;         // kernels one launch of graph_exec runs
   DevSession graph_dev{};              // kernel parameter the graph was captured with
   size_t cap_mut = 0, cap_imm = 0, cap_dec = 0;   // capacities of the device / pinned buffers (reused across loads)
 };
@@ -170,20 +169,19 @@ cudaError_t launch_visit(Kernel k, uint32_t grid, size_t smem, cudaStream_t st, 
 }
 
 // The per-visit launches of one link of the visit chain (allocate view, or backfill with `backfill`), in the class record type CR
-// of the session.  `pdl`: launch with programmatic dependent launch (graph capture); `extra` counts the prepass launches.
+// of the session.  `prepass`: the inter-pod affinity priority's passes first; `pdl`: programmatic dependent launch (graph capture).
 template <class CR>
-cudaError_t launch_visit_link(kb_engine* e, const DevSession& D, const bool backfill, const bool pdl, uint32_t* extra) {
+cudaError_t launch_visit_link(kb_engine* e, RecTag<CR>, const DevSession& D, const bool backfill, const bool prepass, const bool pdl) {
   if (D.aff.on) {
     // inter-pod affinity: the priority's passes over the feasible nodes (they return at once for a class without a weight
-    // list), then the visit with predicate step 10 / the score term in its scan.  nodeorder is off in backfill: no passes
+    // list), then the visit with predicate step 10 / the score term in its scan
     if (backfill) { visit_kernel<1, 1, CR><<<e->scan_grid, SCAN_THREADS, e->visit_smem, e->stream>>>(D); return cudaGetLastError(); }
-    if (D.aff.has_weights || D.aff.has_pref) {
+    if (prepass) {
       const uint32_t ag = std::max(1u, std::min((e->N + AFF_THREADS - 1) / AFF_THREADS, (uint32_t)e->sm_count * 4u));
       const uint32_t ag1 = std::max(1u, std::min((e->N + AFF_THREADS / 32 - 1) / (AFF_THREADS / 32), (uint32_t)e->sm_count * 8u));   // pass 1: a warp per node
       aff_prepass_kernel<0, CR><<<ag, AFF_THREADS, 0, e->stream>>>(D);
       aff_prepass_kernel<1, CR><<<ag1, AFF_THREADS, 0, e->stream>>>(D);
       aff_prepass_kernel<2, CR><<<ag, AFF_THREADS, 0, e->stream>>>(D);
-      if (extra) *extra += 3;
     }
     return launch_visit(visit_kernel<0, 1, CR>, e->scan_grid, e->visit_smem, e->stream, D, pdl);
   }
@@ -194,18 +192,38 @@ cudaError_t launch_visit_link(kb_engine* e, const DevSession& D, const bool back
   return launch_visit(visit_kernel<0, 0, CR>, e->scan_grid, e->visit_smem, e->stream, D, pdl);
 }
 
+// Enqueues n links of the visit chain: the per-visit launches and, sharded without peer memory, the all-gather of every rank's top-32
+// keys and node records and the identical replay.  Returns KB_OK with *kernels = the kernels enqueued, or the failure (e->err).
+int enqueue_links(kb_engine* e, const DevSession& D, const bool backfill, const bool pdl, const uint32_t n, uint32_t* kernels) {
+  const bool prepass = D.aff.on && !backfill && (D.aff.has_weights || D.aff.has_pref);   // nodeorder is off in backfill: no passes
+  const bool gather = e->world > 1 && !D.p2p && !e->replicated;     // a replicated rank replays in visit_kernel itself (DevSession.world == 1)
+  for (uint32_t i = 0; i < n; ++i) {
+    CUDA_TRY(e, with_rec(e->built.rec, [&](auto t) { return launch_visit_link(e, t, D, backfill, prepass, pdl); }));
+    if (gather) {
+      const int rc = g_nccl.AllGather(D.sendbuf, D.recvbuf, (size_t)xchg_u64(e->ncols), kNcclUint64, e->comm, e->stream);
+      if (rc != 0) return fail(e, KB_E_NCCL, "ncclAllGather: %s", g_nccl.GetErrorString(rc));
+      if (backfill) replay_kernel<1><<<1, 64, e->replay_smem, e->stream>>>(D);
+      else replay_kernel<0><<<1, 64, e->replay_smem, e->stream>>>(D);
+    }
+  }
+  CUDA_TRY(e, cudaGetLastError());
+  *kernels = n * ((prepass ? 4u : 1u) + (gather ? 1u : 0u));
+  return KB_OK;
+}
+
+static_assert(std::is_same<ClassRec, ClassRecNarrow>::value, "RecKind::Own runs the kernels' default (narrow) instances");
 // the wide and wide-atom instances' staging buffers (scan_tpi) fit next to their VisitSmem, down to the widest record at one tile
-// per iteration
-static_assert(((sizeof(VisitSmem<ClassRecWide>) + 127) / 128) * 128 + 160 * 1024 <= 227 * 1024, "wide VisitSmem + scan_tpi budget");
-static_assert(((sizeof(VisitSmem<ClassRecWide>) + 127) / 128) * 128 + 2 * (size_t)max_cols<ClassRecWide>() * TILE_NODES * 8 <= 227 * 1024,
-              "wide VisitSmem + two tiles of the widest record");
-static_assert(((sizeof(VisitSmem<ClassRecAtoms>) + 127) / 128) * 128 + 160 * 1024 <= 227 * 1024, "wide-atom VisitSmem + scan_tpi budget");
-static_assert(((sizeof(VisitSmem<ClassRecAtoms>) + 127) / 128) * 128 + 2 * (size_t)max_cols<ClassRecAtoms>() * TILE_NODES * 8 <= 227 * 1024,
-              "wide-atom VisitSmem + two tiles of the widest record");
+// per iteration: the scan_tpi budget and two tiles of the widest record
+template <class CR>
+constexpr bool visit_smem_fits() {
+  return ((sizeof(VisitSmem<CR>) + 127) / 128) * 128 + std::max<size_t>(160 * 1024, 2 * (size_t)max_cols<CR>() * TILE_NODES * 8) <= 227 * 1024;
+}
+static_assert(visit_smem_fits<ClassRecWide>(), "wide VisitSmem + scan_tpi budget / two tiles of the widest record");
+static_assert(visit_smem_fits<ClassRecAtoms>(), "wide-atom VisitSmem + scan_tpi budget / two tiles of the widest record");
 
 // Shared-memory sizes and limits of the kernels of class record type CR for a session with B.tpi staged tiles of e->tile_smem bytes
 template <class CR>
-cudaError_t set_kernel_smem(kb_engine* e, const uint32_t tpi, const uint32_t kchain) {
+cudaError_t set_kernel_smem(kb_engine* e, RecTag<CR>, const uint32_t tpi, const uint32_t kchain) {
   e->visit_smem = ((sizeof(VisitSmem<CR>) + 127) / 128) * 128 + 2 * (size_t)tpi * e->tile_smem;
   cudaError_t c = cudaSuccess;
   for (const void* k : {(const void*)visit_kernel<0, 0, CR>, (const void*)visit_kernel<1, 0, CR>, (const void*)visit_kernel<0, 1, CR>,
@@ -402,14 +420,15 @@ int kb_session_load(kb_engine* e, const kb_snapshot* s, const kb_plugin_conf* co
   {
     // the chain kernel keeps K class records, K lists and the fold buffers next to the tile staging buffers: when that
     // does not fit into shared memory for this record width, fall back to fewer classes per launch
-    const size_t tile_b = (size_t)tile_ncols(s ? s->R : 2, s ? s->W : 1) * TILE_NODES * 8;
-    const uint32_t tpi = scan_tpi(s ? s->R : 2, s ? s->W : 1);
+    const uint32_t R = s ? s->R : 2, W = s ? s->W : 1;
+    const size_t tile_b = (size_t)tile_ncols(R, W) * TILE_NODES * 8;
+    const uint32_t tpi = scan_tpi(R, W);
     const size_t lim = 227 * 1024;
-    const bool wide = s && s->R > KB_NARROW_R, atoms = s && s->W > KB_NARROW_W;
-    const size_t h4 = wide ? chain_smem_header<4, ClassRecWide>() : atoms ? chain_smem_header<4, ClassRecAtoms>() : chain_smem_header<4>();
-    const size_t h2 = wide ? chain_smem_header<2, ClassRecWide>() : atoms ? chain_smem_header<2, ClassRecAtoms>() : chain_smem_header<2>();
-    if (kchain == 4 && h4 + 2 * tpi * tile_b > lim) kchain = 2;
-    if (kchain == 2 && h2 + 2 * tpi * tile_b > lim) kchain = 1;
+    with_rec(rec_kind(R, W), [&](auto t) {
+      using CR = typename decltype(t)::type;
+      if (kchain == 4 && chain_smem_header<4, CR>() + 2 * tpi * tile_b > lim) kchain = 2;
+      if (kchain == 2 && chain_smem_header<2, CR>() + 2 * tpi * tile_b > lim) kchain = 1;
+    });
   }
   // world > 1: by default every rank runs the whole cycle on the full (replicated) node table — the cycle is bound by the
   // serial replay, not by the scan, so sharding the scan only adds an exchange per visit (DESIGN.md §6); KB_ENGINE_SHARD
@@ -419,7 +438,7 @@ int kb_session_load(kb_engine* e, const kb_snapshot* s, const kb_plugin_conf* co
   const bool aff_session = s && s->pod_affinity != nullptr;
   // more resource dimensions or mask words than the sharded exchange's records carry (P2P_RANK_U64): replicated unless
   // KB_ENGINE_SHARD asks for the sharded path, which such sessions refuse (kb_build.h)
-  const bool wide_session = s && (s->R > KB_NARROW_R || s->W > KB_NARROW_W);
+  const bool wide_session = s && rec_kind(s->R, s->W) != RecKind::Own;
   const bool pipe_ok = e->pipe_req && e->coop_ok;
   const bool pipe_try = (pipe_ok && (e->world == 1 || !e->shard_req)) || ((aff_session || wide_session) && !e->shard_req);      // = the full table on this rank
   int rc_build = build_session(s, conf, (uint32_t)std::max(1, e->sm_count), B, &be, pipe_try ? 0u : (uint32_t)e->rank,
@@ -482,10 +501,7 @@ int kb_session_load(kb_engine* e, const kb_snapshot* s, const kb_plugin_conf* co
   e->job_min_avail_host = B.job_min_avail;
   e->scan_grid = grid;
   e->tile_smem = tile_u64 * 8;
-  e->wide = R > KB_NARROW_R;
-  e->atoms = W > KB_NARROW_W;
-  CUDA_TRY(e, e->wide ? set_kernel_smem<ClassRecWide>(e, B.tpi, B.kchain)
-              : e->atoms ? set_kernel_smem<ClassRecAtoms>(e, B.tpi, B.kchain) : set_kernel_smem<ClassRecNarrow>(e, B.tpi, B.kchain));
+  CUDA_TRY(e, with_rec(B.rec, [&](auto t) { return set_kernel_smem(e, t, B.tpi, B.kchain); }));
   // the cycle is a chain of identical launches: capture BATCH of them into one graph (one host call per batch)
   e->replay_smem = ((sizeof(VisitSmem<>) + 127) / 128) * 128;
   CUDA_TRY(e, cudaFuncSetAttribute(replay_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)e->replay_smem));
@@ -503,21 +519,10 @@ int kb_session_load(kb_engine* e, const kb_snapshot* s, const kb_plugin_conf* co
   }
   if (!e->dev.pipe && (!e->graph_exec || memcmp(&e->graph_dev, &e->dev, sizeof(DevSession)) != 0)) {
     free_graph(e);
-    // the cycle is a chain of identical launches: capture BATCH of them into one graph (one host call per batch).
-    // Sharded: scan shard -> ncclAllGather (top-32 keys + node records per rank) -> identical replay on every rank.
-    const size_t cnt = (size_t)xchg_u64(e->ncols);
+    // the cycle is a chain of identical launches: capture BATCH of them into one graph (one host call per batch)
     cudaError_t ce = cudaStreamBeginCapture(e->stream, cudaStreamCaptureModeThreadLocal);
-    bool ok = ce == cudaSuccess;
-    for (uint32_t i = 0; ok && i < BATCH; ++i) {
-      const bool pdl = e->pdl && (e->world == 1 || e->replicated);
-      if (e->wide) ok = launch_visit_link<ClassRecWide>(e, e->dev, false, pdl, nullptr) == cudaSuccess;
-      else if (e->atoms) ok = launch_visit_link<ClassRecAtoms>(e, e->dev, false, pdl, nullptr) == cudaSuccess;
-      else ok = launch_visit_link<ClassRecNarrow>(e, e->dev, false, pdl, nullptr) == cudaSuccess;
-      if (e->world > 1 && !e->dev.p2p && !e->replicated) {      // a replicated rank replays in visit_kernel itself (DevSession.world == 1)
-        ok = g_nccl.AllGather(e->dev.sendbuf, e->dev.recvbuf, cnt, kNcclUint64, e->comm, e->stream) == 0;
-        replay_kernel<0><<<1, 64, e->replay_smem, e->stream>>>(e->dev);
-      }
-    }
+    const bool pdl = e->pdl && (e->world == 1 || e->replicated);
+    bool ok = ce == cudaSuccess && enqueue_links(e, e->dev, false, pdl, BATCH, &e->graph_launches) == KB_OK;
     cudaGraph_t g = nullptr;
     ce = cudaStreamEndCapture(e->stream, &g);
     ok = ok && ce == cudaSuccess && g != nullptr;
@@ -593,23 +598,11 @@ int run_action(kb_engine* e, const bool backfill, kb_decision* out, kb_stats* st
       launches += 1;
     } else if (use_graph) {
       CUDA_TRY(e, cudaGraphLaunch(e->graph_exec, e->stream));
-      launches += ((D.aff.on && (D.aff.has_weights || D.aff.has_pref)) ? 4 : (e->world == 1 || D.p2p || e->replicated) ? 1 : 2) * BATCH;
+      launches += e->graph_launches;
     } else {
-      // sharded node axis without peer memory: scan shard -> all-gather (top-32 keys + node records per rank) -> identical replay
-      const size_t cnt = (size_t)xchg_u64(e->ncols);
-      for (uint32_t i = 0; i < batch; ++i) {
-        if (e->wide) CUDA_TRY(e, launch_visit_link<ClassRecWide>(e, D, backfill, false, &launches));
-        else if (e->atoms) CUDA_TRY(e, launch_visit_link<ClassRecAtoms>(e, D, backfill, false, &launches));
-        else CUDA_TRY(e, launch_visit_link<ClassRecNarrow>(e, D, backfill, false, &launches));
-        if (e->world > 1 && !D.p2p && !e->replicated) {
-          int rc = g_nccl.AllGather(D.sendbuf, D.recvbuf, cnt, kNcclUint64, e->comm, e->stream);
-          if (rc != 0) return fail(e, KB_E_NCCL, "ncclAllGather: %s", g_nccl.GetErrorString(rc));
-          if (backfill) replay_kernel<1><<<1, 64, e->replay_smem, e->stream>>>(D);
-          else replay_kernel<0><<<1, 64, e->replay_smem, e->stream>>>(D);
-        }
-      }
-      CUDA_TRY(e, cudaGetLastError());
-      launches += ((e->world == 1 || D.p2p || e->replicated) ? 1 : 2) * batch;
+      uint32_t kernels = 0;
+      if (const int rc = enqueue_links(e, D, backfill, false, batch, &kernels)) return rc;
+      launches += kernels;
     }
     CUDA_TRY(e, cudaMemcpyAsync(e->h_ctl, D.ctl, sizeof(Ctl), cudaMemcpyDeviceToHost, e->stream));
     if (use_pipe && e->watchdog_s > 0) {
@@ -931,9 +924,9 @@ int kb_predicate_score(kb_engine* e, uint32_t task_lo, uint32_t task_hi, uint8_t
   }
   dim3 grid(e->NT, (task_hi - task_lo + MATRIX_TASKS_PER_CTA - 1) / MATRIX_TASKS_PER_CTA);
   cudaEventRecord(e->ev0, e->stream);
-  if (e->wide) matrix_kernel<ClassRecWide><<<grid, MATRIX_THREADS, e->tile_smem, e->stream>>>(e->dev, e->d_task_class, task_lo, task_hi, d_fit, d_score);
-  else if (e->atoms) matrix_kernel<ClassRecAtoms><<<grid, MATRIX_THREADS, e->tile_smem, e->stream>>>(e->dev, e->d_task_class, task_lo, task_hi, d_fit, d_score);
-  else matrix_kernel<<<grid, MATRIX_THREADS, e->tile_smem, e->stream>>>(e->dev, e->d_task_class, task_lo, task_hi, d_fit, d_score);
+  with_rec(e->built.rec, [&](auto t) {
+    matrix_kernel<typename decltype(t)::type><<<grid, MATRIX_THREADS, e->tile_smem, e->stream>>>(e->dev, e->d_task_class, task_lo, task_hi, d_fit, d_score);
+  });
   cudaEventRecord(e->ev1, e->stream);
   cudaError_t c = cudaGetLastError();
   if (c == cudaSuccess && fit) c = cudaMemcpyAsync(fit, d_fit, n, cudaMemcpyDeviceToHost, e->stream);
@@ -962,9 +955,9 @@ int kb_best_nodes(kb_engine* e, uint32_t task_lo, uint32_t task_hi, uint64_t* be
     uint32_t chunks = std::max(1u, std::min(n, (uint32_t)(8 * e->sm_count + e->NT - 1) / std::max(1u, e->NT)));
     dim3 grid(e->NT, chunks);
     cudaEventRecord(e->ev0, e->stream);
-    if (e->wide) best_nodes_kernel<ClassRecWide><<<grid, MATRIX_THREADS, e->tile_smem, e->stream>>>(e->dev, e->d_task_class, task_lo, task_hi, d_best);
-    else if (e->atoms) best_nodes_kernel<ClassRecAtoms><<<grid, MATRIX_THREADS, e->tile_smem, e->stream>>>(e->dev, e->d_task_class, task_lo, task_hi, d_best);
-    else best_nodes_kernel<<<grid, MATRIX_THREADS, e->tile_smem, e->stream>>>(e->dev, e->d_task_class, task_lo, task_hi, d_best);
+    with_rec(e->built.rec, [&](auto t) {
+      best_nodes_kernel<typename decltype(t)::type><<<grid, MATRIX_THREADS, e->tile_smem, e->stream>>>(e->dev, e->d_task_class, task_lo, task_hi, d_best);
+    });
     cudaEventRecord(e->ev1, e->stream);
     c = cudaGetLastError();
   }

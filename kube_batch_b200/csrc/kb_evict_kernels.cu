@@ -33,6 +33,7 @@ namespace kb {
 
 constexpr int EVICT_THREADS = 512;
 constexpr uint32_t EVICT_EXIT = 0xFFFFFFFFu;
+static_assert(std::is_same<ClassRec, ClassRecNarrow>::value, "RecKind::Own runs the kernels' default (narrow) instances");
 
 __device__ __forceinline__ uint32_t ev_ld_acquire(const uint32_t* p) {
   uint32_t v; asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory"); return v;
@@ -284,20 +285,14 @@ cudaError_t launch_evict(const bool preempt, const DevSession& S, const EvictDev
   if (c != cudaSuccess) return c;
   c = cudaMemsetAsync(reinterpret_cast<char*>(E.ctl) + offsetof(EvictCtl, cls_valid), 0, 4, stream);
   if (c != cudaSuccess) return c;
-  // a session with more resource dimensions or mask words than the narrow class record holds runs the wide or the wide-atom
-  // instances (kb_build.h)
-  const bool wide = S.cf.R > KB_NARROW_R, atoms = S.cf.W > KB_NARROW_W;
-  if (S.J) {
-    if (wide) evict_scan_kernel<ClassRecWide><<<(S.J + 255) / 256, 256, 0, stream>>>(S, E);
-    else if (atoms) evict_scan_kernel<ClassRecAtoms><<<(S.J + 255) / 256, 256, 0, stream>>>(S, E);
-    else evict_scan_kernel<><<<(S.J + 255) / 256, 256, 0, stream>>>(S, E);
-  }
   DevSession s = S; EvictDev ev = E;
   void* args[] = {(void*)&s, (void*)&ev};
-  const void* fn = wide ? (preempt ? (const void*)evict_kernel<1, ClassRecWide> : (const void*)evict_kernel<0, ClassRecWide>)
-                 : atoms ? (preempt ? (const void*)evict_kernel<1, ClassRecAtoms> : (const void*)evict_kernel<0, ClassRecAtoms>)
-                         : (preempt ? (const void*)evict_kernel<1> : (const void*)evict_kernel<0>);
-  return cudaLaunchCooperativeKernel(fn, dim3(workers + 1), dim3(EVICT_THREADS), args, 0, stream);
+  return with_rec(rec_kind(S.cf.R, S.cf.W), [&](auto t) {
+    using CR = typename decltype(t)::type;
+    if (S.J) evict_scan_kernel<CR><<<(S.J + 255) / 256, 256, 0, stream>>>(S, E);
+    const void* fn = preempt ? (const void*)evict_kernel<1, CR> : (const void*)evict_kernel<0, CR>;
+    return cudaLaunchCooperativeKernel(fn, dim3(workers + 1), dim3(EVICT_THREADS), args, 0, stream);
+  });
 }
 
 }  // namespace kb
